@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py — frames/sec of the Self-Forcing hot path on B200 (BASELINE.json metric).
+"""bench.py — frames/sec of the Self-Forcing hot path on one H100 (BASELINE.json metric).
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference]
 
@@ -57,9 +57,9 @@ def measured_peaks():
     p = ROOT / "MEASURED_PEAKS.json"
     if p.exists():
         j = json.loads(p.read_text())
-        return {"tensor": j.get("bf16_tflops_sustained", 1425.5), "hbm": j.get("hbm_gbs", 6480.8),
+        return {"tensor": j.get("bf16_tflops_sustained", 989.0), "hbm": j.get("hbm_gbs", 3350.0),
                 "source": "MEASURED_PEAKS.json (sustained cuBLAS bf16; kernel timed inside a long step)"}
-    return {"tensor": 1400.0, "hbm": 6650.0, "source": "fallback of B200_PROFILING.md"}
+    return {"tensor": 989.0, "hbm": 3350.0, "source": "H100 SXM data sheet (dense bf16, HBM3) at a 700 W power limit"}
 
 
 # ---------------------------------------------------------------------------------------------
@@ -251,8 +251,17 @@ def emit(line: dict):
         os.write(_JSON_FD, data)
 
 
-def _flat_roofline(prof: dict, ms_step: float, peaks: dict, traffic_db: dict) -> dict:
-    """roofline object for the dominant kernel family (the tcgen05 GEMMs) + flat per-kernel scalars.
+def dump_frames(out_dir: str, px: torch.Tensor) -> None:
+    """What a caller of the timed path receives from its last step: the decoded block, [1, 12, 3, 480, 832] fp32
+    (57.5 MB), as out_dir/frames.npy.  Weights, prompt, noise and latents are seeded, so equal arguments give equal
+    inputs from run to run."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    np.save(os.path.join(out_dir, "frames.npy"), px.float().cpu().numpy())
+
+
+def _flat_roofline(prof: dict, ms_step: float, peaks: dict) -> dict:
+    """roofline object for the dominant kernel family (the wgmma GEMMs) + flat per-kernel scalars.
     ``prof`` comes from ONE separately profiled step (CUDA events around every launch of a family), never from the
     timed region; ``share`` = family time / that step's time."""
     def fam(name):
@@ -262,7 +271,8 @@ def _flat_roofline(prof: dict, ms_step: float, peaks: dict, traffic_db: dict) ->
         return g["flops"] / (g["ms"] * 1e-3) / 1e12, g["ms"] / ms_step, g["n"]
     gem, gem_share, gem_n = fam("gemm")
     out = {"bound": "tensor",
-           "kernel": "kr_gemm (tcgen05: gemm2_tn_kernel CTA-pair + gemm_tn_kernel single-CTA, all DiT linears)",
+           "kernel": "kr_gemm (wgmma: gemm2_tn_kernel 2-CTA cluster, gemm_tn_kernel fixed width, gemm_flex_kernel "
+                     "wave-fitted width; all DiT linears)",
            "achieved": gem, "peak": peaks["tensor"], "unit": "TFLOP/s", "frac": (gem / peaks["tensor"]) if gem else None,
            "peak_source": peaks["source"], "launches_timed": gem_n, "share_of_step": gem_share,
            "how": "algorithmic FLOPs of the launches / their CUDA-event time, from one extra profiled step after the "
@@ -277,23 +287,10 @@ def _flat_roofline(prof: dict, ms_step: float, peaks: dict, traffic_db: dict) ->
         out[label + "_share"] = share
         if a is not None:
             by_kernel[label] = {"achieved": a, "frac": a / peaks["tensor"], "launches_timed": n, "share_of_step": share}
-    dominant = max(("gemm2_tn_kernel", "gemm_tn_kernel"),
-                   key=lambda k: (prof.get("gemm/" + k) or {"ms": 0})["ms"])
-    out["traffic"] = traffic_db.get(dominant, {}).get("dram_bytes_per_launch")
-    out["traffic_kernel"] = dominant
+    out["dominant_kernel"] = max(("gemm2_tn_kernel", "gemm_tn_kernel", "gemm_flex_kernel", "gemm_sk_kernel"),
+                                 key=lambda k: (prof.get("gemm/" + k) or {"ms": 0})["ms"])
     out["by_kernel"] = by_kernel
     return out
-
-
-def _traffic_db() -> dict:
-    for name in ("r02_gemm_traffic.json", "r01_gemm_traffic.json"):
-        tp = ROOT / "profiles" / name
-        if tp.exists():
-            try:
-                return json.loads(tp.read_text())
-            except Exception:  # noqa: BLE001
-                pass
-    return {}
 
 
 def _reference_host_egress_ms(px: torch.Tensor, reps: int = 2):
@@ -336,7 +333,7 @@ def assemble_line(args, world, sp_mode, pp_mode, use_graphs, main_run, e2e_run, 
     value = streams * K * FRAMES_PER_STEP / (ms / 1e3)
     e2e = streams * K * FRAMES_PER_STEP / (e2e_run["ms"] / 1e3)
     peaks = measured_peaks()
-    roofline = _flat_roofline(main_run["prof"], main_run["ms_prof"], peaks, _traffic_db())
+    roofline = _flat_roofline(main_run["prof"], main_run["ms_prof"], peaks)
     block_tflop = (4 * LAYERS * layer_flops(LQ, LKV) + LAYERS * layer_flops(LQ, LQ)) / 1e12 * (args.layers / LAYERS)
     if pp_mode:
         par = (f"ONE stream on {world} GPUs, DiT layers sharded {LAYERS}/{world} per GPU (BASELINE configs[2]): residual "
@@ -412,6 +409,8 @@ def run_vae_workload(args, dev, rank, world, barrier, max_over_ranks):
         launches = ops.launch_count - n0
         clk = clocks.stop() if rank == 0 else None
         ms = max_over_ranks(e0.elapsed_time(e1))
+        if args.dump_outputs and rank == 0:
+            dump_frames(args.dump_outputs, px)
         # one profiled step (per-launch events) for the conv family's TF/s
         ops.profile_begin()
         p0, p1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
@@ -447,13 +446,6 @@ def run_vae_workload(args, dev, rank, world, barrier, max_over_ranks):
     # (fully fused) = feature-cache read+write 3.8 GB + pixels 57.5 MB + weights 146.6 MB = 4.0 GB
     ALG_UNFUSED, ALG_FUSED = 24.1e9, 4.0e9
     gbs = ALG_UNFUSED / (ms / K * 1e-3) / 1e9
-    vt = {}
-    tp = ROOT / "profiles" / "r02_vae_traffic.json"
-    if tp.exists():
-        try:
-            vt = json.loads(tp.read_text())
-        except Exception:  # noqa: BLE001
-            vt = {}
     line = {"metric": "vae_decode_frames_per_second_832x480", "value": world * K * 12 / (ms / 1e3), "unit": "frames/s",
             "n_gpus": world, "steps": K, "warmup": W, "ms_per_step": ms / K, "higher_is_better": True,
             "scaling": "weak", "vs_baseline": None, "dtype": "f16", "data": "synthetic",
@@ -467,12 +459,11 @@ def run_vae_workload(args, dev, rank, world, barrier, max_over_ranks):
                          "achieved": conv_tf, "peak": peaks["tensor"], "unit": "TFLOP/s",
                          "frac": conv_tf / peaks["tensor"] if conv_tf else None, "peak_source": peaks["source"],
                          "share_of_step": vcv["ms"] / ms_prof if ms_prof > 0 else None, "launches_timed": vcv["n"],
-                         "traffic": vt.get("dram_bytes_per_block"),
+
                          "hbm": {"algorithmic_gb_per_block_unfused": ALG_UNFUSED / 1e9,
                                  "algorithmic_gb_per_block_fully_fused": ALG_FUSED / 1e9,
                                  "achieved_gbs_vs_unfused_bytes": gbs, "peak_gbs": peaks["hbm"],
-                                 "frac_of_hbm_peak": gbs / peaks["hbm"],
-                                 "measured_dram_gb_per_block": (vt.get("dram_bytes_per_block") or 0) / 1e9 or None}},
+                                 "frac_of_hbm_peak": gbs / peaks["hbm"]}},
             "cpu_baseline": None}
     emit(line)
 
@@ -483,6 +474,9 @@ def main():
     ap.add_argument("--gpus", type=int, default=1)
     ap.add_argument("--steps", type=int, default=4)
     ap.add_argument("--warmup", type=int, default=3)
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the last timed step's decoded frames to DIR/frames.npy (float32); "
+                         "block and vae_decode workloads")
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
     ap.add_argument("--parallel", default="sp", choices=["replicas", "sp", "pp"],
                     help="N>1 headline: ONE stream sequence-parallel over all GPUs (default, strong scaling; "
@@ -506,6 +500,8 @@ def main():
     world = int(os.environ.get("WORLD_SIZE", "1"))
     local = int(os.environ.get("LOCAL_RANK", "0"))
     if args.impl == "reference":
+        if args.dump_outputs:
+            raise SystemExit("--dump-outputs writes what the timed device path computed; --impl reference has none")
         run_reference_arm(args, rank, world)
         return
     if args.warmup < 3:
@@ -608,6 +604,7 @@ def main():
             out["ms"] = max_over_ranks(e0.elapsed_time(e1))
             if decode:
                 assert px.shape == (1, 12, 3, 480, 832) and px.dtype == torch.float32
+                out["px"] = px.clone()
             if profile_step:
                 barrier()
                 ops.profile_begin()
@@ -677,6 +674,8 @@ def main():
 
     streams = 1 if sp_mode else world           # independent video streams in flight
     main_run = measure(sp_mode, K, 42, profile_step=True)
+    if args.dump_outputs and rank == 0:
+        dump_frames(args.dump_outputs, main_run["px"])
     e2e_run = measure_e2e(sp_mode, K, 1042)
 
     # same end-to-end loop with the byte egress kernel (SURVEY.md 8f.2): kr_frames_to_rgb8 does the reference's
@@ -707,7 +706,7 @@ def main():
             egress_jpeg = {"value": None, "error": f"{type(ex).__name__}: {ex}"[:200]}
 
     # FP8 tier (SURVEY.md 8f.4; the reference's `enable_fp8: true`): same loop with the DiT block linears on the
-    # kind::f8f6f4 GEMM + dynamic per-tensor activation casts.  Reported beside the bf16 headline, never instead of it.
+    # e4m3 wgmma GEMM + dynamic per-tensor activation casts.  Reported beside the bf16 headline, never instead of it.
     fp8_line = None
     if world == 1 and not args.no_fp8:
         from realtime_video_b200 import fp8 as fp8mod

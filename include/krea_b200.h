@@ -1,4 +1,4 @@
-/* krea_b200.h — C ABI of libkrea_b200.so (B200 / sm_100a kernels for the Self-Forcing
+/* krea_b200.h — C ABI of libkrea_b200.so (H100 / sm_90a kernels for the Self-Forcing
  * causal-inference hot path of krea-ai/realtime-video).
  *
  * The reference has no FFI of its own (it is pure Python over torch; SURVEY.md §8b), so this
@@ -44,7 +44,7 @@ const char* kr_last_error(void);
 #define KR_EPI_F32 4           /* out(fp32) = (acc + bias) * alpha                               */
 #define KR_EPI_MUL 5           /* out = cast(cast(acc + bias) * res)  (UMT5 gated FFN, t5.py:138-140) */
 
-/* out[M,N] = epilogue(a[M,K] @ w[N,K]^T + bias[N]); tcgen05/TMEM tensor-core GEMM.
+/* out[M,N] = epilogue(a[M,K] @ w[N,K]^T + bias[N]); wgmma tensor-core GEMM.
  * Replaces nn.Linear (cuBLASLt) + the elementwise ops that follow it:
  *   to_qkv / q / k / v / o      wan/modules/causal_model.py:246-253, :396
  *   gate + residual             wan/modules/causal_model.py:476, :487-488
@@ -78,7 +78,7 @@ size_t kr_gemm_workspace_bytes(void);
  * a dynamic per-tensor e4m3 cast of its input followed by an FP8 matmul with fp32 accumulation and bf16 output.
  *   kr_fp8_quantize : x [rows, cols] bf16 -> q e4m3 bytes [rows, ldq] = sat(x * 448 / amax(|x|)); state (2 floats of
  *                     device memory) receives [amax, amax / 448]; &state[1] is the scale_a of the following GEMM.
- *   kr_gemm_fp8     : out = epilogue((a_q @ w_q^T) * (*scale_a) * scale_w + bias), tcgen05.mma.kind::f8f6f4, bf16
+ *   kr_gemm_fp8     : out = epilogue((a_q @ w_q^T) * (*scale_a) * scale_w + bias), e4m3 wgmma, bf16
  *                     output, the epilogues of kr_gemm except KR_EPI_F32 / KR_EPI_MUL; N % 256 == 0, K % 16 == 0.
  * Weights are quantised once by the caller (w_q = sat(w * 448 / amax(|w|)), scale_w = amax / 448). */
 int kr_fp8_quantize(const void* x, int ldx, int rows, int cols, void* q, int ldq, float* state, void* stream);
@@ -87,8 +87,8 @@ int kr_gemm_fp8(int epilogue, const void* a, int lda, const void* w, int ldw, co
                 const void* gate, int gate_stride, int rows_per_gate, void* out2, int ldc2, int n_split, int row_offset,
                 void* stream);
 
-/* Which kernel kr_gemm launches for this epilogue and shape: 1 = the single-CTA kernel, 2 = the CTA-pair
- * kernel (tcgen05.mma.cta_group::2, 256x256 tiles), 3 = the stream-K kernel (only with a workspace), 4 = the
+/* Which kernel kr_gemm launches for this epilogue and shape: 1 = the single-CTA kernel, 2 = the 2-CTA
+ * cluster kernel (128x256 tile per CTA, W multicast to both), 3 = the stream-K kernel (only with a workspace), 4 = the
  * single-CTA kernel with a runtime tile width fitted to whole waves of SMs (small-M shards).  Host-only
  * queries (no launch), used by bench.py to attribute launch time per kernel. */
 int kr_gemm_kernel_id(int epilogue, int M, int N, int K);
@@ -174,7 +174,7 @@ int kr_unpatchify_x0(const void* head_out, int ldh, const void* xt, const double
 
 /* ---- causal 3D VAE decoder (channels-last activations [frames, H, W, C], fp16 or bf16) ---- */
 
-/* CausalConv3d / Conv2d / 1x1x1 conv as a tcgen05 implicit GEMM (wan/modules/vae.py:17-36,
+/* CausalConv3d / Conv2d / 1x1x1 conv as a wgmma implicit GEMM (wan/modules/vae.py:17-36,
  * :175-209; demo_utils/vae_block3.py:46-91, :386-443).  `in` holds t_in >= T + kt - 1 frames:
  * the (kt-1) cached frames in front of the T new ones (read in place, no cat/pad); spatial zero
  * padding is the TMA out-of-bounds fill.  weight: [w_rows, kt*kh*kw*cin] (tap-major, cin

@@ -1,6 +1,6 @@
 """ctypes binding of libkrea_b200.so (the C ABI declared in include/krea_b200.h).
 
-The library is built in-tree by :func:`build` (``nvcc -gencode arch=compute_100a,code=sm_100a``)
+The library is built in-tree by :func:`build` (``nvcc -gencode arch=compute_90a,code=sm_90a``)
 so the ``.so`` travels with the repository snapshot.  There is no CPU or eager fallback: every
 op raises if the library is missing or a call returns a non-zero code (the reference's error
 convention is plain Python exceptions, SURVEY.md §8b).
@@ -19,7 +19,7 @@ LIB_PATH = _PKG_DIR / "libkrea_b200.so"
 SOURCES = ["kr_host.cu", "kr_gemm.cu", "kr_gemm2.cu", "kr_gemm_sk.cu", "kr_gemm_fp8.cu", "kr_attn.cu", "kr_t5attn.cu", "kr_dit_elem.cu", "kr_vae.cu", "kr_jpeg.cu", "kr_dit_block.cu", "kr_api.cu"]
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
     "--shared", "-Xcompiler", "-fPIC", "-cudart", "static",
 ]
 
@@ -52,7 +52,7 @@ def needs_build() -> bool:
 
 
 def build(force: bool = False, verbose: bool = False) -> Path:
-    """Compile every CUDA source into libkrea_b200.so for sm_100a (cross-compiles without a GPU)."""
+    """Compile every CUDA source into libkrea_b200.so for sm_90a (cross-compiles without a GPU)."""
     with _lock:
         if not force and not needs_build():
             return LIB_PATH
@@ -60,7 +60,7 @@ def build(force: bool = False, verbose: bool = False) -> Path:
         procs = []
         build_dir = _PKG_DIR / "build"
         build_dir.mkdir(exist_ok=True)
-        base = [_nvcc(), "-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo",
+        base = [_nvcc(), "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo",
                 "-std=c++17", "-Xcompiler", "-fPIC"]
         for src in _sources():
             obj = build_dir / (src.stem + ".o")
@@ -74,7 +74,7 @@ def build(force: bool = False, verbose: bool = False) -> Path:
             if verbose and out:
                 print(out.decode(errors="replace"))
         tmp = LIB_PATH.with_suffix(".so.tmp")
-        link = [_nvcc(), "-gencode", "arch=compute_100a,code=sm_100a", "--shared", "-cudart",
+        link = [_nvcc(), "-gencode", "arch=compute_90a,code=sm_90a", "--shared", "-cudart",
                 "static", "-o", str(tmp)] + [str(o) for o in objs]
         r = subprocess.run(link, stdout=subprocess.PIPE, stderr=subprocess.STDOUT)
         if r.returncode != 0:

@@ -1,4 +1,4 @@
-// kr_attn.cu — tcgen05/TMEM flash-attention forward for sm_100a, head_dim 128.
+// kr_attn.cu — wgmma flash-attention forward for sm_90a, head_dim 128.
 //
 //   O[q, h, :] = softmax_k( scale * Q[q, h, :] . K[k, h, :] ) V[k, h, :]
 //
@@ -10,33 +10,13 @@
 // Layout is the reference's [L, heads, 128] (row pitch = heads*128 elements), K/V read in place
 // from the rolling cache tensors.
 //
-// CTA = 256 query rows of one head (two 128-row tiles, "ping-pong"): while softmax warpgroup 0
-// works on S0 the tensor core runs P1.V and Q1.K^T for warpgroup 1 and vice versa.
-//   warp 0        : TMA producer (Q once, K/V ring of 32 KB stages)
-//   warp 1        : tcgen05.mma issuer
-//   warps 4..7    : softmax warpgroup 0 (one thread per query row)
-//   warps 8..11   : softmax warpgroup 1
-// TMEM (512 cols): S0 [0,128) S1 [128,256) O0 [256,384) O1 [384,512); P (16-bit) aliases the
-// first 64 columns of its S buffer and feeds the P.V MMA as the TMEM A operand.
+// CTA = 128 query rows of one head:
+//   warps 0..3    : consumer warpgroup 0 (query rows 0..63):  S = Q.K^T (wgmma, SS), online softmax in
+//                   registers, O += P.V (wgmma, P from registers, V MN-major from shared memory)
+//   warps 4..7    : consumer warpgroup 1 (query rows 64..127)
+//   warps 8..11   : TMA producer warpgroup (warp 8: Q once, K/V ring of 32 KB stages K0 V0 K1 V1 ...)
+// The two consumer warpgroups run out of step, so one's softmax overlaps the other's MMAs.
 // Online softmax with lazy rescaling (O is only rescaled when the running max grows by > 2^8).
-// P is handed to the MMA warp in kParts column slices (one mbarrier each, one elected arrive per warp):
-// P.V over the first keys of a tile can start while the warpgroup still exponentiates the rest.
-// The TMA and MMA roles run in ONE elected thread each (elect.sync, not `lane == 0`: ptxas then emits
-// UTCHMMA / UTCBAR / UTMALDG back to back instead of wrapping each in an ELECT/branch loop).
-//
-// Where the time goes (ncu, Lq 4680 / Lkv 9360 / 40 heads, r01): tensor pipe 58 %, XU (MUFU) 59 %,
-// ~3440 clk per 128 keys against 2048 clk of MMA and 2048 clk of MUFU work.  The two warpgroups are a
-// two-customer closed queue over two servers (MUFU 16 ex2/clk/SM, tensor pipe) plus ~700 clk of
-// per-tile latency (TMEM load, max, store, barrier round trips); mean-value analysis of that queue
-// gives 3500 clk.  Variants measured on B200 and NOT kept (git history has them):
-//   * 1 / 2 / 4 hand-over slices: 1125 / 1128 / 1129 TF/s;  f32x2-packed FFMA/FADD: 1091 TF/s
-//   * quarter of the exponentials as an FMA-pipe cubic (FlashAttention-4 style): 966 TF/s
-//   * fp16 P with ex2.approx.f16x2: SASS is MUFU.EX2.F16 per element (no MUFU saving)
-//   * one 128-row tile per CTA, S double-buffered, warpgroups splitting each tile by columns
-//     (named barrier per tile): 1021 TF/s — the barrier puts both warps of a scheduler in lock step,
-//     so their MUFU phases coincide instead of interleaving, and K/V L2->SM traffic doubles
-//   * two tiles per CTA, 64-key tiles with two S buffers per tile (softmax never waits for P.V):
-//     1052 TF/s — 24 MMAs of 32-64 clk per 64 keys make the single issuing thread the limiter
 #include "kr_common.cuh"
 #include "kr_ops.h"
 
@@ -53,9 +33,7 @@ static constexpr int kKvStages = 4;
 static constexpr int kTileBytes = kTileKV * kHeadDim * 2;   // 32 KB
 static constexpr int kHalfBytes = kTileBytes / 2;           // one 64-column swizzle panel
 static constexpr int kAttnThreads = 384;
-static constexpr int kAttnSmem = 2 * kTileBytes + kKvStages * kTileBytes + 1024 + 256;
-
-static constexpr int kParts = 2;   // P hand-over slices (1, 2 and 4 measured within 0.5 % of each other)
+static constexpr int kAttnSmem = kTileBytes + kKvStages * kTileBytes + 1024 + 256;
 
 template <bool kBf16>
 __global__ void __launch_bounds__(kAttnThreads, 1)
@@ -64,373 +42,204 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
                                              ~static_cast<uintptr_t>(1023));
-  uint8_t* smem_q = smem;                          // 2 tiles
-  uint8_t* smem_kv = smem + 2 * kTileBytes;        // kKvStages tiles
+  uint8_t* smem_q = smem;                          // [2 panels][128 rows][128 B]
+  uint8_t* smem_kv = smem + kTileBytes;            // kKvStages tiles
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem_kv + kKvStages * kTileBytes);
   uint64_t* q_full = bars;                 // [1]
   uint64_t* kv_full = bars + 1;            // [kKvStages]
   uint64_t* kv_empty = kv_full + kKvStages;   // [kKvStages]
-  uint64_t* s_full = kv_empty + kKvStages;    // [2]
-  uint64_t* p_ready = s_full + 2;          // [2][kParts]
-  uint64_t* o_final = p_ready + 2 * kParts;   // [1]
-  uint64_t* o_done = o_final + 1;             // [1] single-tile mode: one phase per P.V(j)
-  uint32_t* tmem_base_smem = reinterpret_cast<uint32_t*>(o_done + 1);
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
-  // linear CTA order: every two-tile CTA of every head first, the single-tile ones (if the last
-  // 256-row block of a head holds <= 128 rows) last, so they fill the tail of the final wave
-  const int nqb = (p.Lq + 2 * kTileQ - 1) / (2 * kTileQ);
-  const bool has_short = (p.Lq - (nqb - 1) * 2 * kTileQ) <= kTileQ;
-  const int full_per_head = has_short ? nqb - 1 : nqb;
-  int head, qb;
-  if (static_cast<int>(blockIdx.x) < p.heads * full_per_head) {
-    head = blockIdx.x / full_per_head;
-    qb = blockIdx.x % full_per_head;
-  } else {
-    head = blockIdx.x - p.heads * full_per_head;
-    qb = nqb - 1;
-  }
-  const int q0 = qb * 2 * kTileQ;
+  const int nqb = (p.Lq + kTileQ - 1) / kTileQ;
+  const int head = blockIdx.x / nqb;
+  const int q0 = (blockIdx.x % nqb) * kTileQ;
 
   // number of KV tiles this CTA visits
   int kv_limit = p.Lkv;
   if (p.mask_mode == 1) {
-    int last_q = q0 + 2 * kTileQ - 1;
+    int last_q = q0 + kTileQ - 1;
     if (last_q > p.Lq - 1) last_q = p.Lq - 1;
     const int hi = (last_q / p.block_len + 1) * p.block_len;
     if (hi < kv_limit) kv_limit = hi;
   }
   const int n_tiles = (kv_limit + kTileKV - 1) / kTileKV;
-  // second 128-row query tile entirely past Lq (last CTA of a head): its MMAs / softmax are skipped
-  const bool two = (q0 + kTileQ) < p.Lq;
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 256) {
     prefetch_tmap(&tmap_q);
     prefetch_tmap(&tmap_k);
     prefetch_tmap(&tmap_v);
-  }
-  if (warp == 1) {
-    if (lane == 0) {
-      mbar_init(q_full, 1);
-      for (int i = 0; i < kKvStages; ++i) {
-        mbar_init(&kv_full[i], 1);
-        mbar_init(&kv_empty[i], 1);
-      }
-      for (int i = 0; i < 2; ++i) {
-        mbar_init(&s_full[i], 1);
-        for (int q = 0; q < kParts; ++q) mbar_init(&p_ready[i * kParts + q], 4);   // one arrive per warp
-      }
-      mbar_init(o_final, 1);
-      mbar_init(o_done, 1);
-      fence_barrier_init();
+    mbar_init(q_full, 1);
+    for (int i = 0; i < kKvStages; ++i) {
+      mbar_init(&kv_full[i], 1);
+      mbar_init(&kv_empty[i], 2);   // one arrive per consumer warpgroup
     }
-    __syncwarp();
-    tmem_alloc<512>(tmem_base_smem);
+    fence_barrier_init();
   }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_base_smem;
 
-  if (warp == 0) {
+  // ring items: K_j = 2j, V_j = 2j + 1
+  auto st = [](int item) { return item % kKvStages; };
+  auto ph = [](int item) { return static_cast<uint32_t>((item / kKvStages) & 1); };
+
+  if (warp >= 8) {
     // ===================== TMA producer =====================
-    if (elect_one()) {
+    producer_regs();
+    if (warp == 8 && elect_one()) {
       const int col = head * kHeadDim;
-      mbar_expect_tx(q_full, 2 * kTileBytes);
-      for (int t = 0; t < 2; ++t)
-        for (int h = 0; h < 2; ++h)
-          tma_load_2d(smem_q + t * kTileBytes + h * kHalfBytes, &tmap_q, q_full, col + h * 64,
-                      q0 + t * kTileQ);
-      int stage = 0;
-      uint32_t phase = 0;
-      // ring order: K0 V0 K1 V1 ...
+      mbar_expect_tx(q_full, kTileBytes);
+      for (int h = 0; h < 2; ++h) tma_load_2d(smem_q + h * kHalfBytes, &tmap_q, q_full, col + h * 64, q0);
       for (int it = 0; it < 2 * n_tiles; ++it) {
         const int j = it >> 1;
         const CUtensorMap* tm = (it & 1) ? &tmap_v : &tmap_k;
-        mbar_wait(&kv_empty[stage], phase ^ 1);
-        mbar_expect_tx(&kv_full[stage], kTileBytes);
+        mbar_wait(&kv_empty[st(it)], ph(it) ^ 1);
+        mbar_expect_tx(&kv_full[st(it)], kTileBytes);
         for (int h = 0; h < 2; ++h)
-          tma_load_2d(smem_kv + stage * kTileBytes + h * kHalfBytes, tm, &kv_full[stage],
-                      col + h * 64, j * kTileKV);
-        if (++stage == kKvStages) {
-          stage = 0;
-          phase ^= 1;
-        }
+          tma_load_2d(smem_kv + st(it) * kTileBytes + h * kHalfBytes, tm, &kv_full[st(it)], col + h * 64,
+                      j * kTileKV);
       }
     }
-  } else if (warp == 1) {
-    // ===================== MMA issuer =====================
-    constexpr uint32_t idesc_qk = make_idesc<kBf16>(128, 128, 0, 0);   // A,B K-major
-    // P.V: A = P from TMEM (KV dtype), B = V MN-major in the KV dtype
-    constexpr uint32_t idesc_pv = make_idesc_ab(128, 128, kBf16 ? 1u : 0u, kBf16 ? 1u : 0u, 0, 1);
-    const uint32_t q_addr = smem_u32(smem_q);
-    const uint32_t kv_addr = smem_u32(smem_kv);
-    const uint32_t tS[2] = {tmem_base + 0, tmem_base + 128};
-    const uint32_t tO[2] = {tmem_base + 256, tmem_base + 384};
+    return;
+  }
 
-    // S buffer `sb` = Q tile `qt` . K(stage)^T
-    auto issue_qk = [&](int qt, int sb, int stage) {
-      const uint32_t a = q_addr + qt * kTileBytes;
-      const uint32_t b = kv_addr + stage * kTileBytes;
+  // ===================== consumer warpgroups =====================
+  consumer_regs();
+  const int wg = warp >> 2;
+  const bool leader = (threadIdx.x & 127) == 0;
+  const uint32_t q_addr = smem_u32(smem_q) + wg * 64 * 128;
+  const uint32_t kv_addr = smem_u32(smem_kv);
+  // this thread's two query rows (fragment rows lane/4 and lane/4 + 8 of its warp's 16)
+  int q_row[2], row_hi[2], row_lo[2], n_phantom[2];
+#pragma unroll
+  for (int r = 0; r < 2; ++r) {
+    q_row[r] = q0 + wg * 64 + (warp & 3) * 16 + (lane >> 2) + 8 * r;
+    row_hi[r] = p.Lkv;
+    row_lo[r] = 0;
+    n_phantom[r] = 0;
+    if (p.mask_mode == 1) {
+      const int qq = q_row[r] < p.Lq ? q_row[r] : p.Lq - 1;
+      const int hi = (qq / p.block_len + 1) * p.block_len;
+      if (p.window > 0) row_lo[r] = hi - p.window > 0 ? hi - p.window : 0;
+      if (hi < row_hi[r]) row_hi[r] = hi;
+      if (hi > p.Lkv) n_phantom[r] = hi - p.Lkv < p.pad_keys ? hi - p.Lkv : p.pad_keys;
+    }
+  }
+  float m_run[2] = {-INFINITY, -INFINITY};
+  float l_run[2] = {0.f, 0.f};     // this thread's partial row sums (its 2 columns of every 8)
+  const float sl2 = p.scale_log2;
+  float o[kHeadDim / 2];
+#pragma unroll
+  for (int i = 0; i < kHeadDim / 2; ++i) o[i] = 0.f;
+
+  mbar_wait(q_full, 0);
+  for (int j = 0; j < n_tiles; ++j) {
+    // ---- S = Q . K_j^T ----
+    float s[kTileKV / 2];
+    mbar_wait(&kv_full[st(2 * j)], ph(2 * j));
+    {
+      const uint32_t b = kv_addr + st(2 * j) * kTileBytes;
+      wgmma_fence();
 #pragma unroll
       for (int k = 0; k < kHeadDim / 16; ++k) {
         const uint32_t off = (k >> 2) * kHalfBytes + (k & 3) * 32;
-        umma_ss(tS[sb], make_smem_desc(a + off, 16, 1024), make_smem_desc(b + off, 16, 1024),
-                idesc_qk, k != 0 ? 1u : 0u);
+        wgmma_ss<kTileKV, kBf16, 0>(s, make_smem_desc(q_addr + off, 16, 1024), make_smem_desc(b + off, 16, 1024),
+                                    k != 0 ? 1 : 0);
       }
-    };
-    // O buffer `ob` += P (16-bit, aliasing S buffer `sb`) . V(stage); each slice of P is consumed as
-    // soon as its mbarrier (phase `par`) completes.
-    auto issue_pv = [&](int ob, int sb, int stage, bool first, uint32_t par) {
-      const uint32_t b = kv_addr + stage * kTileBytes;
-      constexpr int kSteps = kTileKV / 16 / kParts;
-#pragma unroll
-      for (int part = 0; part < kParts; ++part) {
-        mbar_wait(&p_ready[sb * kParts + part], par);
-        tc_fence_after();
-#pragma unroll
-        for (int kk = 0; kk < kSteps; ++kk) {
-          const int k = part * kSteps + kk;
-          // P: 16 keys = 8 TMEM columns per k-step; V: 16 key rows of 128 B per panel
-          umma_ts(tO[ob], tS[sb] + k * 8, make_smem_desc(b + k * 2048, kHalfBytes, 1024), idesc_pv,
-                  (first && k == 0) ? 0u : 1u);
-        }
-      }
-    };
-    // ring items: K_j = 2j, V_j = 2j + 1
-    auto st = [](int item) { return item % kKvStages; };
-    auto ph = [](int item) { return static_cast<uint32_t>((item / kKvStages) & 1); };
-
-    // one thread runs the whole issue loop (waits included): no warp-wide polling next to the softmax
-    // warps that share this scheduler
-    if (elect_one()) {
-      mbar_wait(q_full, 0);
-      if (two) {
-        // ---- two query tiles: ping-pong between the softmax warpgroups ----
-        mbar_wait(&kv_full[st(0)], ph(0));
-        tc_fence_after();
-        issue_qk(0, 0, st(0));
-        umma_commit(&s_full[0]);
-        issue_qk(1, 1, st(0));
-        umma_commit(&s_full[1]);
-        umma_commit(&kv_empty[st(0)]);
-        for (int j = 0; j < n_tiles; ++j) {
-          const int vi = 2 * j + 1, ki = 2 * j + 2;
-          const bool more = (j + 1 < n_tiles);
-          mbar_wait(&kv_full[st(vi)], ph(vi));   // V_j
-          issue_pv(0, 0, st(vi), j == 0, j & 1);
-          if (more) {
-            mbar_wait(&kv_full[st(ki)], ph(ki));   // K_{j+1}
-            tc_fence_after();
-            issue_qk(0, 0, st(ki));
-            umma_commit(&s_full[0]);
-          }
-          issue_pv(1, 1, st(vi), j == 0, j & 1);
-          umma_commit(&kv_empty[st(vi)]);
-          if (more) {
-            issue_qk(1, 1, st(ki));
-            umma_commit(&s_full[1]);
-            umma_commit(&kv_empty[st(ki)]);
-          }
-        }
-      } else {
-        // ---- one query tile (last CTA of a head): S double-buffered so Q.K_{j+1}^T overlaps softmax(j) ----
-        mbar_wait(&kv_full[st(0)], ph(0));
-        tc_fence_after();
-        issue_qk(0, 0, st(0));
-        umma_commit(&s_full[0]);
-        umma_commit(&kv_empty[st(0)]);
-        if (n_tiles > 1) {
-          mbar_wait(&kv_full[st(2)], ph(2));
-          tc_fence_after();
-          issue_qk(0, 1, st(2));
-          umma_commit(&s_full[1]);
-          umma_commit(&kv_empty[st(2)]);
-        }
-        for (int j = 0; j < n_tiles; ++j) {
-          const int vi = 2 * j + 1, ki = 2 * (j + 2);
-          const int sb = j & 1;
-          mbar_wait(&kv_full[st(vi)], ph(vi));   // V_j
-          issue_pv(0, sb, st(vi), j == 0, (j >> 1) & 1);
-          umma_commit(&kv_empty[st(vi)]);
-          umma_commit(o_done);
-          if (j + 2 < n_tiles) {
-            mbar_wait(&kv_full[st(ki)], ph(ki));   // K_{j+2}
-            tc_fence_after();
-            issue_qk(0, sb, st(ki));
-            umma_commit(&s_full[sb]);
-            umma_commit(&kv_empty[st(ki)]);
-          }
-        }
-      }
-      umma_commit(o_final);
+      wgmma_commit();
+      wgmma_wait<0>();
+      reg_fence(s);
     }
-    __syncwarp();
-  } else if (warp >= 4 && (two || warp < 8)) {
-    // ===================== softmax warpgroups =====================
-    const int wg = (warp - 4) >> 2;
-    const int quarter = warp & 3;
-    const int row_in_tile = quarter * 32 + lane;
-    const int q_row = q0 + wg * kTileQ + row_in_tile;
-    const uint32_t lane_off = static_cast<uint32_t>(quarter * 32) << 16;
-    const uint32_t tS_base = tmem_base + lane_off;
-    const uint32_t tO = tmem_base + lane_off + 256 + wg * 128;
+    if (leader) mbar_arrive(&kv_empty[st(2 * j)]);
 
-    int row_hi = p.Lkv, row_lo = 0;
-    int n_phantom = 0;
-    if (p.mask_mode == 1) {
-      const int qq = q_row < p.Lq ? q_row : p.Lq - 1;
-      const int hi = (qq / p.block_len + 1) * p.block_len;
-      if (p.window > 0) row_lo = hi - p.window > 0 ? hi - p.window : 0;
-      if (hi < row_hi) row_hi = hi;
-      if (hi > p.Lkv) n_phantom = hi - p.Lkv < p.pad_keys ? hi - p.Lkv : p.pad_keys;
-    }
-
-    float m_run = -INFINITY;
-    float l_run = 0.f;
-    const float sl2 = p.scale_log2;
-
-    for (int j = 0; j < n_tiles; ++j) {
-      // two tiles: S buffer = warpgroup, one completion per KV tile; one tile: buffers alternate
-      const int sb = two ? wg : (j & 1);
-      const uint32_t par = two ? static_cast<uint32_t>(j & 1) : static_cast<uint32_t>((j >> 1) & 1);
-      const uint32_t tS = tS_base + sb * 128;
-      mbar_wait(&s_full[sb], par);
-      tc_fence_after();
-      uint32_t r0[32], r1[32], r2[32], r3[32];
-      tmem_ld_x32(tS + 0, r0);
-      tmem_ld_x32(tS + 32, r1);
-      tmem_ld_x32(tS + 64, r2);
-      tmem_ld_x32(tS + 96, r3);
-      tmem_ld_wait();
-
-      const int hi = row_hi - j * kTileKV;
-      const int lo = row_lo - j * kTileKV;
+    // ---- mask, running max, lazy rescale ----
+    float nms[2];
+#pragma unroll
+    for (int r = 0; r < 2; ++r) {
+      const int hi = row_hi[r] - j * kTileKV, lo = row_lo[r] - j * kTileKV;
       if (hi < kTileKV || lo > 0) {
 #pragma unroll
-        for (int c = 0; c < 32; ++c) {
-          if (c >= hi || c < lo) r0[c] = 0xff800000u;
-          if (c + 32 >= hi || c + 32 < lo) r1[c] = 0xff800000u;
-          if (c + 64 >= hi || c + 64 < lo) r2[c] = 0xff800000u;
-          if (c + 96 >= hi || c + 96 < lo) r3[c] = 0xff800000u;
-        }
+        for (int nb = 0; nb < kTileKV / 8; ++nb)
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            const int c = nb * 8 + 2 * (lane & 3) + e;
+            if (c >= hi || c < lo) s[4 * nb + 2 * r + e] = -INFINITY;
+          }
       }
       float mt = -INFINITY;
 #pragma unroll
-      for (int c = 0; c < 32; ++c) {
-        mt = fmaxf(mt, fmaxf(fmaxf(__uint_as_float(r0[c]), __uint_as_float(r1[c])),
-                             fmaxf(__uint_as_float(r2[c]), __uint_as_float(r3[c]))));
-      }
-      const float m_new = fmaxf(m_run, mt);
-      const bool need = (m_new - m_run) * sl2 > 8.0f;   // also true when m_run == -inf
-      const float m_used = need ? m_new : m_run;
-      const float alpha = need ? fast_exp2((m_run - m_new) * sl2) : 1.0f;
-      if (j > 0 && __any_sync(0xffffffffu, need)) {
-        // rescale this row's O accumulator in TMEM.  Two-tile mode: s_full(j) was committed after
-        // P.V(j-1) in issue order, so O is quiescent.  Single-tile mode: Q.K^T(j) is issued BEFORE
-        // P.V(j-1) (other S buffer), so wait for that P.V's own commit (phases j-1 or j complete).
-        if (!two) {
-          mbar_wait(o_done, static_cast<uint32_t>((j - 1) & 1));
-          tc_fence_after();
-        }
-#pragma unroll 1
-        for (int c = 0; c < 4; ++c) {
-          uint32_t o[32];
-          tmem_ld_x32(tO + c * 32, o);
-          tmem_ld_wait();
+      for (int nb = 0; nb < kTileKV / 8; ++nb) mt = fmaxf(mt, fmaxf(s[4 * nb + 2 * r], s[4 * nb + 2 * r + 1]));
+      mt = fmaxf(mt, __shfl_xor_sync(0xffffffffu, mt, 1));
+      mt = fmaxf(mt, __shfl_xor_sync(0xffffffffu, mt, 2));
+      const float m_new = fmaxf(m_run[r], mt);
+      const bool need = (m_new - m_run[r]) * sl2 > 8.0f;   // also true when m_run == -inf
+      const float m_used = need ? m_new : m_run[r];
+      const float alpha = need ? fast_exp2((m_run[r] - m_new) * sl2) : 1.0f;
+      if (need && j > 0) {
 #pragma unroll
-          for (int i = 0; i < 32; ++i) o[i] = __float_as_uint(__uint_as_float(o[i]) * alpha);
-          tmem_st_x32(tO + c * 32, o);
+        for (int nb = 0; nb < kHeadDim / 8; ++nb) {
+          o[4 * nb + 2 * r] *= alpha;
+          o[4 * nb + 2 * r + 1] *= alpha;
         }
       }
-      l_run *= alpha;
-      m_run = m_used;
+      l_run[r] *= alpha;
+      m_run[r] = m_used;
       // a row whose every visible key so far is masked (local window) keeps m = -inf: use 0
-      const float nms = (m_used == -INFINITY) ? 0.f : -m_used * sl2;
-      float rowsum = 0.f;
-      // exponentiate one 32-key quarter of the row into 16 packed columns
-      auto quarter_exp = [&](const uint32_t (&r)[32], uint32_t* pk) {
+      nms[r] = (m_used == -INFINITY) ? 0.f : -m_used * sl2;
+    }
+    // ---- P = exp2(S * scale_log2 - m), packed as the A operand of P.V ----
+    uint32_t pa[kTileKV / 16][4];
 #pragma unroll
-        for (int c = 0; c < 16; ++c) {
-          const float a0 = fast_exp2(fmaf(__uint_as_float(r[2 * c]), sl2, nms));
-          const float a1 = fast_exp2(fmaf(__uint_as_float(r[2 * c + 1]), sl2, nms));
-          rowsum += a0 + a1;
-          pk[c] = kBf16 ? pack_bf16x2(a0, a1) : pack_f16x2(a0, a1);
+    for (int kk = 0; kk < kTileKV / 16; ++kk) {
+#pragma unroll
+      for (int h = 0; h < 2; ++h)
+#pragma unroll
+        for (int r = 0; r < 2; ++r) {
+          const int i = 8 * kk + 4 * h + 2 * r;
+          const float a0 = fast_exp2(fmaf(s[i], sl2, nms[r]));
+          const float a1 = fast_exp2(fmaf(s[i + 1], sl2, nms[r]));
+          l_run[r] += a0 + a1;
+          pa[kk][2 * h + r] = kBf16 ? pack_bf16x2(a0, a1) : pack_f16x2(a0, a1);
         }
-      };
-      // tcgen05.wait::st is warp-wide (.sync.aligned): once it returns every lane's slice of P is in
-      // TMEM, so one elected arrive per warp publishes it
-      auto hand_over = [&](int part) {
-        tmem_st_wait();
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&p_ready[sb * kParts + part]);
-      };
-      if constexpr (kParts == 4) {
-        uint32_t pk[16];
-        quarter_exp(r0, pk); tmem_st_x16(tS + 0, pk); hand_over(0);
-        quarter_exp(r1, pk); tmem_st_x16(tS + 16, pk); hand_over(1);
-        quarter_exp(r2, pk); tmem_st_x16(tS + 32, pk); hand_over(2);
-        quarter_exp(r3, pk); tmem_st_x16(tS + 48, pk); hand_over(3);
-      } else {
-        uint32_t pk[32];
-        quarter_exp(r0, pk);
-        quarter_exp(r1, pk + 16);
-        tmem_st_x32(tS + 0, *reinterpret_cast<const uint32_t(*)[32]>(&pk[0]));
-        if constexpr (kParts == 2) hand_over(0);
-        quarter_exp(r2, pk);
-        quarter_exp(r3, pk + 16);
-        tmem_st_x32(tS + 32, *reinterpret_cast<const uint32_t(*)[32]>(&pk[0]));
-        hand_over(kParts - 1);
-      }
-      l_run += rowsum;
     }
-
-    // ---- epilogue: O / l -> global ----
-    mbar_wait(o_final, 0);
-    tc_fence_after();
-    float o_scale = 1.0f;
-    if (n_phantom > 0) {
-      // phantom keys: score 0, value 0 -> only the softmax denominator (and max) see them
-      const float m_fin = fmaxf(m_run, 0.f);
-      o_scale = fast_exp2((m_run - m_fin) * sl2);
-      l_run = l_run * o_scale + static_cast<float>(n_phantom) * fast_exp2(-m_fin * sl2);
-    }
-    const float inv_l = o_scale / l_run;
-    const bool row_ok = q_row < p.Lq;
-    uint16_t* orow = reinterpret_cast<uint16_t*>(p.out) + static_cast<size_t>(row_ok ? q_row : 0) * p.ldo +
-                     head * kHeadDim;
-#pragma unroll 1
-    for (int c = 0; c < 4; ++c) {
-      uint32_t o[32];
-      tmem_ld_x32(tO + c * 32, o);
-      tmem_ld_wait();
-      if (row_ok) {
+    // ---- O += P . V_j ----
+    mbar_wait(&kv_full[st(2 * j + 1)], ph(2 * j + 1));
+    {
+      const uint32_t b = kv_addr + st(2 * j + 1) * kTileBytes;
+      wgmma_fence();
 #pragma unroll
-        for (int q = 0; q < 4; ++q) {
-          uint4 w;
-          float f[8];
-#pragma unroll
-          for (int i = 0; i < 8; ++i) f[i] = __uint_as_float(o[q * 8 + i]) * inv_l;
-          if (kBf16) {
-            w.x = pack_bf16x2(f[0], f[1]); w.y = pack_bf16x2(f[2], f[3]);
-            w.z = pack_bf16x2(f[4], f[5]); w.w = pack_bf16x2(f[6], f[7]);
-          } else {
-            w.x = pack_f16x2(f[0], f[1]); w.y = pack_f16x2(f[2], f[3]);
-            w.z = pack_f16x2(f[4], f[5]); w.w = pack_f16x2(f[6], f[7]);
-          }
-          *reinterpret_cast<uint4*>(orow + c * 32 + q * 8) = w;
-        }
-      }
+      for (int kk = 0; kk < kTileKV / 16; ++kk)
+        // V: 16 key rows of 128 B per panel, the next 64 head dims one panel (kHalfBytes) further
+        wgmma_rs<kHeadDim, kBf16>(o, pa[kk], make_smem_desc(b + kk * 2048, kHalfBytes, 1024), 1);
+      wgmma_commit();
+      wgmma_wait<0>();
+      reg_fence(o);
     }
+    if (leader) mbar_arrive(&kv_empty[st(2 * j + 1)]);
   }
 
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc<512>(tmem_base);
+  // ---- epilogue: O / l -> global ----
+#pragma unroll
+  for (int r = 0; r < 2; ++r) {
+    float l = l_run[r];
+    l += __shfl_xor_sync(0xffffffffu, l, 1);
+    l += __shfl_xor_sync(0xffffffffu, l, 2);
+    float o_scale = 1.0f;
+    if (n_phantom[r] > 0) {
+      // phantom keys: score 0, value 0 -> only the softmax denominator (and max) see them
+      const float m_fin = fmaxf(m_run[r], 0.f);
+      o_scale = fast_exp2((m_run[r] - m_fin) * sl2);
+      l = l * o_scale + static_cast<float>(n_phantom[r]) * fast_exp2(-m_fin * sl2);
+    }
+    const float inv_l = o_scale / l;
+    if (q_row[r] < p.Lq) {
+      uint16_t* orow = reinterpret_cast<uint16_t*>(p.out) + static_cast<size_t>(q_row[r]) * p.ldo +
+                       head * kHeadDim + 2 * (lane & 3);
+#pragma unroll
+      for (int nb = 0; nb < kHeadDim / 8; ++nb) {
+        const float f0 = o[4 * nb + 2 * r] * inv_l, f1 = o[4 * nb + 2 * r + 1] * inv_l;
+        *reinterpret_cast<uint32_t*>(orow + nb * 8) = kBf16 ? pack_bf16x2(f0, f1) : pack_f16x2(f0, f1);
+      }
+    }
   }
 }
 
@@ -470,7 +279,7 @@ int attn_fwd(int dtype, const void* q, int ldq, const void* k, int ldk, const vo
       }
       attr_set[bf ? 0 : 1] = true;
     }
-    dim3 grid(((p.Lq + 2 * kTileQ - 1) / (2 * kTileQ)) * p.heads);
+    dim3 grid(((p.Lq + kTileQ - 1) / kTileQ) * p.heads);
     kern<<<grid, kAttnThreads, kAttnSmem, stream>>>(tq, tk, tv, p);
   }
   cudaError_t e = cudaGetLastError();

@@ -1,8 +1,8 @@
-// kr_common.cuh — sm_100a PTX wrappers shared by every kernel in this library.
+// kr_common.cuh — sm_90a PTX wrappers shared by every kernel in this library.
 //
-// Only inline PTX the Blackwell programming model needs: mbarrier, TMA
-// (cp.async.bulk.tensor), tcgen05 (alloc / mma / commit / ld / st / fences) and
-// the UMMA shared-memory / instruction descriptors.  No CUTLASS / CuTe.
+// Only inline PTX the Hopper programming model needs: mbarrier, TMA
+// (cp.async.bulk.tensor), wgmma (fence / commit / wait, kr_wgmma.cuh) and the
+// shared-memory matrix descriptors.  No CUTLASS / CuTe.
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_bf16.h>
@@ -11,6 +11,7 @@
 #include <stdint.h>
 
 #include "../../include/krea_b200.h"
+#include "kr_wgmma.cuh"
 
 #define KR_DEVICE __device__ __forceinline__
 
@@ -122,152 +123,83 @@ template <int N>
 KR_DEVICE void tma_store_wait() {
   asm volatile("cp.async.bulk.wait_group %0;" ::"n"(N) : "memory");
 }
-// generic-proxy smem writes -> visible to the async proxy (TMA store / UMMA reads)
+// generic-proxy smem writes -> visible to the async proxy (TMA store / wgmma reads)
 KR_DEVICE void fence_proxy_async_smem() {
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
 }
 
 // ---------------------------------------------------------------------------
-// tcgen05: TMEM allocation
+// clusters: rank, cluster-wide barrier, remote mbarrier arrive, multicast TMA
 // ---------------------------------------------------------------------------
-template <uint32_t kCols>
-KR_DEVICE void tmem_alloc(uint32_t* smem_result) {
-  static_assert(kCols >= 32 && kCols <= 512 && (kCols & (kCols - 1)) == 0, "pow2 in [32,512]");
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(
-                   smem_u32(smem_result)),
-               "n"(kCols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
+KR_DEVICE uint32_t cluster_ctarank() {
+  uint32_t r;
+  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
+  return r;
 }
-template <uint32_t kCols>
-KR_DEVICE void tmem_dealloc(uint32_t taddr) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "n"(kCols)
-               : "memory");
+// every thread of every CTA of the cluster (barrier init visible cluster-wide / no CTA exits while a peer may
+// still multicast into its shared memory or arrive on its barriers)
+KR_DEVICE void cluster_sync() {
+  asm volatile("barrier.cluster.arrive.release;\n\tbarrier.cluster.wait.acquire;" ::: "memory");
 }
-KR_DEVICE void tc_fence_before() {
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
+// arrive on the mbarrier at the same shared-memory offset in CTA `cta` of the cluster
+KR_DEVICE void mbar_arrive_cluster(uint64_t* bar, uint32_t cta) {
+  asm volatile(
+      "{\n\t.reg .b32 ra;\n\t"
+      "mapa.shared::cluster.u32 ra, %0, %1;\n\t"
+      "mbarrier.arrive.release.cluster.shared::cluster.b64 _, [ra];\n\t}" ::"r"(smem_u32(bar)),
+      "r"(cta)
+      : "memory");
 }
-KR_DEVICE void tc_fence_after() {
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
+// the box lands at the same offset in every CTA of `mask`, each CTA's `bar` (same offset) receives the bytes
+KR_DEVICE void tma_load_2d_mc(void* smem_dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1, uint16_t mask) {
+  asm volatile(
+      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster"
+      " [%0], [%1, {%3, %4}], [%2], %5;" ::"r"(smem_u32(smem_dst)),
+      "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "h"(mask)
+      : "memory");
 }
 
 // ---------------------------------------------------------------------------
-// tcgen05: descriptors
+// wgmma (warpgroup MMA, accumulators in registers)
 // ---------------------------------------------------------------------------
-// Shared-memory matrix descriptor (64-bit), sm_100 "version 1":
+// Shared-memory matrix descriptor (64-bit), sm_90:
 //   [0,14)  start address >> 4        [16,30) leading byte offset >> 4
-//   [32,46) stride byte offset >> 4   [46,48) version = 1
-//   [49,52) base offset = 0           [61,64) layout: 0 none, 2 SW128, 4 SW64, 6 SW32
-// K-major SW128 operand: rows of 128 B (64 x 16-bit), 8-row groups 1024 B apart
-//   -> SBO = 1024, LBO unused (set 1).
-// MN-major SW128 operand ([k][mn] with mn contiguous, 64 mn-elements = 128 B per
-//   k-row): 8 k-rows 128 B apart form a 1024 B atom; the next 8 k-rows are SBO
-//   bytes further, the next 64 mn-elements LBO bytes further.
-// layout_type: 2 = SWIZZLE_128B (default), 4 = SWIZZLE_64B, 6 = SWIZZLE_32B, 0 = none
+//   [32,46) stride byte offset >> 4   [62,64) swizzle: 0 none, 1 SW128, 2 SW64, 3 SW32
+// K-major SW128 operand: rows of 128 B (64 x 16-bit), 8-row groups 1024 B apart -> SBO = 1024, LBO unused;
+//   the k-th 16-element step of a 64-wide panel starts 32 B further (the swizzle is applied to absolute
+//   address bits, so tiles must be 1024-byte aligned).
+// MN-major SW128 operand ([k][mn], 64 mn-elements = 128 B per k-row): 8 k-rows form a 1024 B atom; the next
+//   8 k-rows are SBO bytes further, the next 64 mn-elements LBO bytes further.
+enum : uint32_t { kSwz128 = 1, kSwz64 = 2, kSwz32 = 3 };
 KR_DEVICE uint64_t make_smem_desc(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes,
-                                  uint32_t layout_type = 2) {
+                                  uint32_t swizzle = kSwz128) {
   uint64_t d = 0;
   d |= static_cast<uint64_t>((smem_addr & 0x3FFFF) >> 4);
   d |= static_cast<uint64_t>((lbo_bytes >> 4) & 0x3FFF) << 16;
   d |= static_cast<uint64_t>((sbo_bytes >> 4) & 0x3FFF) << 32;
-  d |= static_cast<uint64_t>(1) << 46;   // version
-  d |= static_cast<uint64_t>(layout_type) << 61;
+  d |= static_cast<uint64_t>(swizzle) << 62;
   return d;
 }
-
-// Instruction descriptor for kind::f16 (32-bit):
-//   [4,6) D fmt (1 = f32)  [7,10) A fmt  [10,13) B fmt (0 = f16, 1 = bf16)
-//   [15] A major (0 = K)   [16] B major (0 = K, 1 = MN)
-//   [17,23) N >> 3         [24,29) M >> 4
-template <bool kBf16>
-__host__ __device__ constexpr uint32_t make_idesc(uint32_t M, uint32_t N, uint32_t a_mn_major,
-                                                  uint32_t b_mn_major) {
-  return (1u << 4) | ((kBf16 ? 1u : 0u) << 7) | ((kBf16 ? 1u : 0u) << 10) | (a_mn_major << 15) |
-         (b_mn_major << 16) | ((N >> 3) << 17) | ((M >> 4) << 24);
+KR_DEVICE void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+KR_DEVICE void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+KR_DEVICE void wgmma_wait() {
+  asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
 }
-
-// same with independent A / B element formats (0 = f16, 1 = bf16)
-__host__ __device__ constexpr uint32_t make_idesc_ab(uint32_t M, uint32_t N, uint32_t a_fmt, uint32_t b_fmt,
-                                                     uint32_t a_mn_major, uint32_t b_mn_major) {
-  return (1u << 4) | (a_fmt << 7) | (b_fmt << 10) | (a_mn_major << 15) | (b_mn_major << 16) |
-         ((N >> 3) << 17) | ((M >> 4) << 24);
+// keep the accumulator registers live and ordered around asynchronous wgmma (no code emitted)
+template <int N>
+KR_DEVICE void reg_fence(float (&d)[N]) {
+#pragma unroll
+  for (int i = 0; i < N; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
-
-// ---------------------------------------------------------------------------
-// tcgen05: mma / commit
-// ---------------------------------------------------------------------------
-// D[tmem] (+)= A[smem] * B[smem]
-KR_DEVICE void umma_ss(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc,
-                       uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t"
-      "}\n" ::"r"(d_tmem),
-      "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-      : "memory");
+// register budget of a warpgroup (all its warps execute it): the TMA warpgroup gives registers back, the
+// consumer warpgroups take them (3 warpgroups: 128 x 40 + 256 x 232 <= 64 K)
+KR_DEVICE void producer_regs() { asm volatile("setmaxnreg.dec.sync.aligned.u32 40;"); }
+KR_DEVICE void consumer_regs() { asm volatile("setmaxnreg.inc.sync.aligned.u32 232;"); }
+// named barrier over `count` threads (the consumer warpgroups of a kernel)
+KR_DEVICE void named_bar_sync(int id, int count) {
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory");
 }
-// D[tmem] (+)= A[tmem] * B[smem]
-KR_DEVICE void umma_ts(uint32_t d_tmem, uint32_t a_tmem, uint64_t b_desc, uint32_t idesc,
-                       uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t"
-      "}\n" ::"r"(d_tmem),
-      "r"(a_tmem), "l"(b_desc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// arrive on an mbarrier once every previously issued tcgen05.mma of this thread retired
-KR_DEVICE void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(
-                   smem_u32(bar))
-               : "memory");
-}
-
-// ---------------------------------------------------------------------------
-// tcgen05: TMEM <-> registers (32 lanes x 32-bit, x8 / x16 / x32 columns)
-// warp w of a warpgroup touches lanes [32*(w%4), 32*(w%4)+32); thread t -> lane
-// ---------------------------------------------------------------------------
-KR_DEVICE void tmem_ld_x32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]),
-        "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]),
-        "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]),
-        "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]),
-        "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-}
-KR_DEVICE void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-
-KR_DEVICE void tmem_st_x32(uint32_t taddr, const uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, "
-      "%17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};" ::"r"(
-          taddr),
-      "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]),
-      "r"(r[8]), "r"(r[9]), "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15]),
-      "r"(r[16]), "r"(r[17]), "r"(r[18]), "r"(r[19]), "r"(r[20]), "r"(r[21]), "r"(r[22]),
-      "r"(r[23]), "r"(r[24]), "r"(r[25]), "r"(r[26]), "r"(r[27]), "r"(r[28]), "r"(r[29]),
-      "r"(r[30]), "r"(r[31])
-      : "memory");
-}
-KR_DEVICE void tmem_st_x16(uint32_t taddr, const uint32_t* r) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16};" ::"r"(taddr),
-      "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]),
-      "r"(r[8]), "r"(r[9]), "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15])
-      : "memory");
-}
-KR_DEVICE void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
 
 // ---------------------------------------------------------------------------
 // numeric helpers

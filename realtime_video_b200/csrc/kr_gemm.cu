@@ -1,9 +1,9 @@
-// kr_gemm.cu — persistent tcgen05/TMEM GEMM for sm_100a.
+// kr_gemm.cu — persistent wgmma GEMM for sm_90a.
 //
 //   C[M,N] = epilogue( A[M,K] @ W[N,K]^T + bias[N] )
 //
 // A and W are row-major with K contiguous (nn.Linear weight layout), 16-bit
-// (bf16 or fp16), accumulation in fp32 in tensor memory.
+// (bf16 or fp16), accumulation in fp32 registers.
 //
 // Replaces, on the reference path, every cuBLASLt call issued by nn.Linear in the
 // DiT block (wan/modules/causal_model.py:246 to_qkv, :396 o, :433-435 ffn;
@@ -11,13 +11,13 @@
 // patch/text/time embeddings; :507 head) together with the elementwise kernels
 // that follow them (bias add, GELU-tanh, per-frame gate, residual add).
 //
-// Structure (one CTA per SM, persistent over output tiles):
-//   warp 0      : TMA producer  (A tile 128x64, W tile BLOCK_Nx64, SWIZZLE_128B)
-//   warp 1      : tcgen05.mma issuer (single elected lane), TMEM allocator
-//   warps 2..5  : epilogue (tcgen05.ld -> registers -> fused math -> global)
-// Pipelines: smem full/empty ring (kStages), TMEM accumulator double buffer
-// (2 x BLOCK_N fp32 columns) so the epilogue of tile i overlaps the mainloop of
-// tile i+1.
+// Structure (one CTA per SM, persistent over 128 x BLOCK_N output tiles):
+//   warps 0..3  : consumer warpgroup 0 (rows 0..63 of the tile): wgmma, then the fused epilogue
+//   warps 4..7  : consumer warpgroup 1 (rows 64..127)
+//   warps 8..11 : TMA producer warpgroup (warp 8: A tile 128x64, W tile BLOCK_Nx64, SWIZZLE_128B), smem
+//                 full/empty ring; it hands most of its registers to the consumers (setmaxnreg)
+// BLOCK_N is a template parameter (the wgmma instruction encodes N); gemm_tn_kernel serves the fixed widths
+// 32..256, gemm_flex_kernel the wave-fitted widths 96..256 whose last column tile may be narrower.
 #include "kr_common.cuh"
 #include "kr_gemm_epi.cuh"
 #include "kr_ops.h"
@@ -29,23 +29,23 @@ namespace kr {
 
 static constexpr int BLOCK_M = 128;
 static constexpr int BLOCK_K = 64;   // 64 x 16-bit = 128 B = one swizzle row
-static constexpr int UMMA_K = 16;
-static constexpr int kNumThreads = 192;
+static constexpr int kNumThreads = 384;
+static constexpr int kSmemBudget = 227 * 1024;
 
 template <int BLOCK_N>
 struct GemmCfg {
   static constexpr int kABytes = BLOCK_M * BLOCK_K * 2;
   static constexpr int kBBytes = BLOCK_N * BLOCK_K * 2;
   static constexpr int kStageBytes = kABytes + kBBytes;
-  static constexpr int kStages = (BLOCK_N == 256) ? 4 : (BLOCK_N == 128 ? 6 : 8);
-  static constexpr int kTmemCols = (2 * BLOCK_N < 32) ? 32 : 2 * BLOCK_N;
-  static constexpr int kSmemBytes = kStages * kStageBytes + 1024 /*align*/ + 256 /*barriers*/;
+  static constexpr int kScrBytes = 8 * kEpiScrFloats * 4;
+  static constexpr int kFit = (kSmemBudget - kScrBytes - 2048) / kStageBytes;
+  static constexpr int kStages = kFit > 8 ? 8 : kFit;
+  static constexpr int kSmemBytes = kStages * kStageBytes + kScrBytes + 1024 /*align*/ + 256 /*barriers*/;
+  static_assert(kStages >= 2, "pipeline needs >= 2 stages");
 };
 
 template <int BLOCK_N, bool kBf16, int kEpi>
-__global__ void __launch_bounds__(kNumThreads, 1)
-gemm_tn_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
-               const GemmParams p) {
+KR_DEVICE void gemm_body(const CUtensorMap* tmap_a, const CUtensorMap* tmap_b, const GemmParams& p) {
   using Cfg = GemmCfg<BLOCK_N>;
   extern __shared__ uint8_t smem_raw[];
   // 1024 B alignment for SWIZZLE_128B tiles
@@ -53,48 +53,33 @@ gemm_tn_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
                                              ~static_cast<uintptr_t>(1023));
   uint8_t* smem_a = smem;
   uint8_t* smem_b = smem + Cfg::kStages * Cfg::kABytes;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + Cfg::kStages * Cfg::kStageBytes);
+  float* scratch = reinterpret_cast<float*>(smem + Cfg::kStages * Cfg::kStageBytes);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + Cfg::kStages * Cfg::kStageBytes + Cfg::kScrBytes);
   uint64_t* full_bar = bars;                       // [kStages]
   uint64_t* empty_bar = bars + Cfg::kStages;       // [kStages]
-  uint64_t* tmem_full = bars + 2 * Cfg::kStages;   // [2]
-  uint64_t* tmem_empty = tmem_full + 2;            // [2]
-  uint32_t* tmem_base_smem = reinterpret_cast<uint32_t*>(tmem_empty + 2);
 
   const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
 
   const int num_m = (p.M + BLOCK_M - 1) / BLOCK_M;
-  const int num_n = p.N / BLOCK_N;
+  const int num_n = (p.N + BLOCK_N - 1) / BLOCK_N;   // last column tile may be narrower (TMA zero-fills, epilogue skips)
   const int num_tiles = num_m * num_n;
   const int num_k = (p.K + BLOCK_K - 1) / BLOCK_K;   // K tail: TMA zero-fills both operands
 
-  if (warp == 0 && lane == 0) {
-    prefetch_tmap(&tmap_a);
-    prefetch_tmap(&tmap_b);
-  }
-  if (warp == 1) {
-    if (lane == 0) {
-      for (int i = 0; i < Cfg::kStages; ++i) {
-        mbar_init(&full_bar[i], 1);
-        mbar_init(&empty_bar[i], 1);
-      }
-      for (int i = 0; i < 2; ++i) {
-        mbar_init(&tmem_full[i], 1);
-        mbar_init(&tmem_empty[i], 4);   // one arrive per epilogue warp
-      }
-      fence_barrier_init();
+  if (threadIdx.x == 256) {
+    prefetch_tmap(tmap_a);
+    prefetch_tmap(tmap_b);
+    for (int i = 0; i < Cfg::kStages; ++i) {
+      mbar_init(&full_bar[i], 1);
+      mbar_init(&empty_bar[i], 2);   // one arrive per consumer warpgroup
     }
-    __syncwarp();
-    tmem_alloc<Cfg::kTmemCols>(tmem_base_smem);
+    fence_barrier_init();
   }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_base_smem;
 
-  if (warp == 0) {
-    // ===================== TMA producer =====================
-    if (elect_one()) {
+  if (warp >= 8) {
+    // ===================== TMA producer (warp 8; warps 9..11 only give their registers back) =====================
+    producer_regs();
+    if (warp == 8 && elect_one()) {
       int stage = 0;
       uint32_t phase = 0;
       for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
@@ -103,9 +88,9 @@ gemm_tn_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
         for (int kb = 0; kb < num_k; ++kb) {
           mbar_wait(&empty_bar[stage], phase ^ 1);
           mbar_expect_tx(&full_bar[stage], Cfg::kStageBytes);
-          tma_load_2d(smem_a + stage * Cfg::kABytes, &tmap_a, &full_bar[stage], kb * BLOCK_K,
+          tma_load_2d(smem_a + stage * Cfg::kABytes, tmap_a, &full_bar[stage], kb * BLOCK_K,
                       m_blk * BLOCK_M);
-          tma_load_2d(smem_b + stage * Cfg::kBBytes, &tmap_b, &full_bar[stage], kb * BLOCK_K,
+          tma_load_2d(smem_b + stage * Cfg::kBBytes, tmap_b, &full_bar[stage], kb * BLOCK_K,
                       n_blk * BLOCK_N);
           if (++stage == Cfg::kStages) {
             stage = 0;
@@ -114,268 +99,41 @@ gemm_tn_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
         }
       }
     }
-  } else if (warp == 1) {
-    // ===================== MMA issuer: ONE thread runs the whole loop =====================
-    // (a warp-wide wait + elect + __syncwarp per k-block left the tensor pipe idle ~25 % of the time:
-    //  the issue loop, not operand delivery, was the limiter — profiles/r01_ncu_gemm_ffn1.txt)
-    if (elect_one()) {
-      constexpr uint32_t idesc = make_idesc<kBf16>(BLOCK_M, BLOCK_N, 0, 0);
-      const uint64_t desc_hi = make_smem_desc(0, 16, 1024) & 0xFFFFFFFF00000000ull;
-      const uint32_t desc_lo_c = static_cast<uint32_t>(make_smem_desc(0, 16, 1024));
-      const uint32_t a0 = smem_u32(smem_a), b0 = smem_u32(smem_b);
-      int stage = 0;
-      uint32_t phase = 0;
-      int acc = 0;
-      uint32_t acc_phase = 0;
-      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-        mbar_wait(&tmem_empty[acc], acc_phase ^ 1);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + acc * BLOCK_N;
-        for (int kb = 0; kb < num_k; ++kb) {
-          mbar_wait(&full_bar[stage], phase);
-          tc_fence_after();
-          const uint32_t a_lo = desc_lo_c | (((a0 + stage * Cfg::kABytes) & 0x3FFFF) >> 4);
-          const uint32_t b_lo = desc_lo_c | (((b0 + stage * Cfg::kBBytes) & 0x3FFFF) >> 4);
-#pragma unroll
-          for (int k = 0; k < BLOCK_K / UMMA_K; ++k) {
-            umma_ss(d_tmem, desc_hi | (a_lo + k * 2), desc_hi | (b_lo + k * 2), idesc, (kb | k) != 0 ? 1u : 0u);
-          }
-          umma_commit(&empty_bar[stage]);          // frees the smem slot when the MMAs retire
-          if (kb == num_k - 1) umma_commit(&tmem_full[acc]);
-          if (++stage == Cfg::kStages) {
-            stage = 0;
-            phase ^= 1;
-          }
-        }
-        if (++acc == 2) {
-          acc = 0;
-          acc_phase ^= 1;
-        }
-      }
-    }
   } else {
-    // ===================== epilogue warps =====================
-    const int quarter = warp & 3;   // TMEM lane quarter this warp may access
-    int acc = 0;
-    uint32_t acc_phase = 0;
+    // ===================== consumer warpgroups =====================
+    consumer_regs();
+    const int wg = warp >> 2;
+    const uint32_t a_base = smem_u32(smem_a) + wg * 64 * 128, b_base = smem_u32(smem_b);
+    float* scr = scratch + warp * kEpiScrFloats;
+    int stage = 0;
+    uint32_t phase = 0;
     for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
       const int m_blk = tile % num_m;
       const int n_blk = tile / num_m;
-      const int row = m_blk * BLOCK_M + quarter * 32 + lane;
-      const bool row_ok = row < p.M;
-      mbar_wait(&tmem_full[acc], acc_phase);
-      tc_fence_after();
-      const uint32_t t_row = tmem_base + (static_cast<uint32_t>(quarter * 32) << 16) + acc * BLOCK_N;
-
-      const uint16_t* gate_row = nullptr;
-      if constexpr (kEpi == EPI_BIAS_GATE_RES) {
-        const int g = row_ok ? (row + p.row_offset) / p.rows_per_gate : 0;
-        gate_row = reinterpret_cast<const uint16_t*>(p.gate) + static_cast<size_t>(g) * p.gate_stride;
-      }
-
-#pragma unroll 1
-      for (int c = 0; c < BLOCK_N / 32; ++c) {
-        uint32_t r[32];
-        tmem_ld_x32(t_row + c * 32, r);
-        tmem_ld_wait();
-        const int col0 = n_blk * BLOCK_N + c * 32;
-        if (c == BLOCK_N / 32 - 1) {
-          // all TMEM reads of this accumulator done -> hand it back to the MMA warp
-          tc_fence_before();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(&tmem_empty[acc]);
-        }
-        if (row_ok) {
-          float v[32];
-#pragma unroll
-          for (int j = 0; j < 32; ++j) v[j] = __uint_as_float(r[j]);
-          gemm_epilogue_row32<kBf16, kEpi>(v, row, col0, p, gate_row);
-        }
-      }
-      if (++acc == 2) {
-        acc = 0;
-        acc_phase ^= 1;
-      }
+      float acc[BLOCK_N / 2];
+      gemm_mainloop<BLOCK_N, kBf16 ? 0 : 1>(acc, a_base, b_base, Cfg::kABytes, Cfg::kBBytes, Cfg::kStages,
+                                            full_bar, empty_bar, stage, phase, 0, num_k);
+      const int n_valid = (p.N - n_blk * BLOCK_N) < BLOCK_N ? (p.N - n_blk * BLOCK_N) : BLOCK_N;
+      gemm_frag_epilogue<BLOCK_N, kBf16, kEpi>(acc, scr, m_blk * BLOCK_M + wg * 64 + (warp & 3) * 16,
+                                               n_blk * BLOCK_N, n_valid, 1.0f, p);
     }
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc<Cfg::kTmemCols>(tmem_base);
   }
 }
 
-// Same kernel with a RUNTIME tile width: lets the planner pick BLOCK_N so that the tile count fills whole waves
-// of SMs (the M = 4680/N-row shards of the multi-GPU mode: 5 row blocks x N/256 column tiles is 2.03 waves for
-// to_qkv, 0.68 of a wave for the N = 5120 projections; 128x192 / 128x176 tiles make that 0.91 / 2.97 waves).
-template <bool kBf16, int kEpi>
+template <int BLOCK_N, bool kBf16, int kEpi>
+__global__ void __launch_bounds__(kNumThreads, 1)
+gemm_tn_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
+               const GemmParams p) {
+  gemm_body<BLOCK_N, kBf16, kEpi>(&tmap_a, &tmap_b, p);
+}
+
+// Same body with a tile width chosen at run time among 96..256 so that the tile count fills whole waves of SMs
+// (the M = 4680/N-row shards of the multi-GPU mode).
+template <int BLOCK_N, bool kBf16, int kEpi>
 __global__ void __launch_bounds__(kNumThreads, 1)
 gemm_flex_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
-                 const GemmParams p, const int BLOCK_N, const int kStages) {
-  // BLOCK_N: runtime tile width (multiple of 32, <= 256); stage = A 16 KB + W BLOCK_N x 128 B
-  const int kABytes = BLOCK_M * BLOCK_K * 2, kBBytes = BLOCK_N * BLOCK_K * 2, kStageBytes = kABytes + kBBytes;
-  extern __shared__ uint8_t smem_raw[];
-  // 1024 B alignment for SWIZZLE_128B tiles
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
-                                             ~static_cast<uintptr_t>(1023));
-  uint8_t* smem_a = smem;
-  uint8_t* smem_b = smem + kStages * kABytes;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + kStages * kStageBytes);
-  uint64_t* full_bar = bars;                       // [kStages]
-  uint64_t* empty_bar = bars + kStages;       // [kStages]
-  uint64_t* tmem_full = bars + 2 * kStages;   // [2]
-  uint64_t* tmem_empty = tmem_full + 2;            // [2]
-  uint32_t* tmem_base_smem = reinterpret_cast<uint32_t*>(tmem_empty + 2);
-
-  const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
-
-  const int num_m = (p.M + BLOCK_M - 1) / BLOCK_M;
-  const int num_n = (p.N + BLOCK_N - 1) / BLOCK_N;   // last column tile may be narrower (TMA zero-fills, epilogue skips)
-  const int num_tiles = num_m * num_n;
-  const int num_k = (p.K + BLOCK_K - 1) / BLOCK_K;   // K tail: TMA zero-fills both operands
-
-  if (warp == 0 && lane == 0) {
-    prefetch_tmap(&tmap_a);
-    prefetch_tmap(&tmap_b);
-  }
-  if (warp == 1) {
-    if (lane == 0) {
-      for (int i = 0; i < kStages; ++i) {
-        mbar_init(&full_bar[i], 1);
-        mbar_init(&empty_bar[i], 1);
-      }
-      for (int i = 0; i < 2; ++i) {
-        mbar_init(&tmem_full[i], 1);
-        mbar_init(&tmem_empty[i], 4);   // one arrive per epilogue warp
-      }
-      fence_barrier_init();
-    }
-    __syncwarp();
-    tmem_alloc<512>(tmem_base_smem);
-  }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_base_smem;
-
-  if (warp == 0) {
-    // ===================== TMA producer =====================
-    if (elect_one()) {
-      int stage = 0;
-      uint32_t phase = 0;
-      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-        const int m_blk = tile % num_m;
-        const int n_blk = tile / num_m;
-        for (int kb = 0; kb < num_k; ++kb) {
-          mbar_wait(&empty_bar[stage], phase ^ 1);
-          mbar_expect_tx(&full_bar[stage], kStageBytes);
-          tma_load_2d(smem_a + stage * kABytes, &tmap_a, &full_bar[stage], kb * BLOCK_K,
-                      m_blk * BLOCK_M);
-          tma_load_2d(smem_b + stage * kBBytes, &tmap_b, &full_bar[stage], kb * BLOCK_K,
-                      n_blk * BLOCK_N);
-          if (++stage == kStages) {
-            stage = 0;
-            phase ^= 1;
-          }
-        }
-      }
-    }
-  } else if (warp == 1) {
-    // ===================== MMA issuer: ONE thread runs the whole loop =====================
-    // (a warp-wide wait + elect + __syncwarp per k-block left the tensor pipe idle ~25 % of the time:
-    //  the issue loop, not operand delivery, was the limiter — profiles/r01_ncu_gemm_ffn1.txt)
-    if (elect_one()) {
-      const uint32_t idesc = make_idesc<kBf16>(BLOCK_M, BLOCK_N, 0, 0);
-      const uint64_t desc_hi = make_smem_desc(0, 16, 1024) & 0xFFFFFFFF00000000ull;
-      const uint32_t desc_lo_c = static_cast<uint32_t>(make_smem_desc(0, 16, 1024));
-      const uint32_t a0 = smem_u32(smem_a), b0 = smem_u32(smem_b);
-      int stage = 0;
-      uint32_t phase = 0;
-      int acc = 0;
-      uint32_t acc_phase = 0;
-      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-        mbar_wait(&tmem_empty[acc], acc_phase ^ 1);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + acc * 256;
-        for (int kb = 0; kb < num_k; ++kb) {
-          mbar_wait(&full_bar[stage], phase);
-          tc_fence_after();
-          const uint32_t a_lo = desc_lo_c | (((a0 + stage * kABytes) & 0x3FFFF) >> 4);
-          const uint32_t b_lo = desc_lo_c | (((b0 + stage * kBBytes) & 0x3FFFF) >> 4);
-#pragma unroll
-          for (int k = 0; k < BLOCK_K / UMMA_K; ++k) {
-            umma_ss(d_tmem, desc_hi | (a_lo + k * 2), desc_hi | (b_lo + k * 2), idesc, (kb | k) != 0 ? 1u : 0u);
-          }
-          umma_commit(&empty_bar[stage]);          // frees the smem slot when the MMAs retire
-          if (kb == num_k - 1) umma_commit(&tmem_full[acc]);
-          if (++stage == kStages) {
-            stage = 0;
-            phase ^= 1;
-          }
-        }
-        if (++acc == 2) {
-          acc = 0;
-          acc_phase ^= 1;
-        }
-      }
-    }
-  } else {
-    // ===================== epilogue warps =====================
-    const int quarter = warp & 3;   // TMEM lane quarter this warp may access
-    int acc = 0;
-    uint32_t acc_phase = 0;
-    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-      const int m_blk = tile % num_m;
-      const int n_blk = tile / num_m;
-      const int row = m_blk * BLOCK_M + quarter * 32 + lane;
-      const bool row_ok = row < p.M;
-      mbar_wait(&tmem_full[acc], acc_phase);
-      tc_fence_after();
-      const uint32_t t_row = tmem_base + (static_cast<uint32_t>(quarter * 32) << 16) + acc * 256;
-      const int n_valid = (p.N - n_blk * BLOCK_N) < BLOCK_N ? (p.N - n_blk * BLOCK_N) : BLOCK_N;
-      const int n_chunks = n_valid / 32;
-
-      const uint16_t* gate_row = nullptr;
-      if constexpr (kEpi == EPI_BIAS_GATE_RES) {
-        const int g = row_ok ? (row + p.row_offset) / p.rows_per_gate : 0;
-        gate_row = reinterpret_cast<const uint16_t*>(p.gate) + static_cast<size_t>(g) * p.gate_stride;
-      }
-
-#pragma unroll 1
-      for (int c = 0; c < n_chunks; ++c) {
-        uint32_t r[32];
-        tmem_ld_x32(t_row + c * 32, r);
-        tmem_ld_wait();
-        const int col0 = n_blk * BLOCK_N + c * 32;
-        if (c == n_chunks - 1) {
-          // all TMEM reads of this accumulator done -> hand it back to the MMA warp
-          tc_fence_before();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(&tmem_empty[acc]);
-        }
-        if (row_ok) {
-          float v[32];
-#pragma unroll
-          for (int j = 0; j < 32; ++j) v[j] = __uint_as_float(r[j]);
-          gemm_epilogue_row32<kBf16, kEpi>(v, row, col0, p, gate_row);
-        }
-      }
-      if (++acc == 2) {
-        acc = 0;
-        acc_phase ^= 1;
-      }
-    }
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc<512>(tmem_base);
-  }
+                 const GemmParams p) {
+  gemm_body<BLOCK_N, kBf16, kEpi>(&tmap_a, &tmap_b, p);
 }
 
 // ---------------------------------------------------------------------------
@@ -401,7 +159,7 @@ static int launch_gemm(const void* a, int lda, const void* w, int ldw, const Gem
     }
     attr_set = true;
   }
-  const int num_tiles = ((p.M + BLOCK_M - 1) / BLOCK_M) * (p.N / BLOCK_N);
+  const int num_tiles = ((p.M + BLOCK_M - 1) / BLOCK_M) * ((p.N + BLOCK_N - 1) / BLOCK_N);
   int grid = sm_count();
   if (grid > num_tiles) grid = num_tiles;
   kern<<<grid, kNumThreads, Cfg::kSmemBytes, stream>>>(ta, tb, p);
@@ -414,11 +172,11 @@ static int launch_gemm(const void* a, int lda, const void* w, int ldw, const Gem
 }
 
 // ---- runtime-width kernel: launcher + width choice -------------------------------------------------
-// Cost model of one 128 x bn tile over one 64-wide k-block, in SM clocks: the MMA takes 2*bn, the operand fetch
-// (128 + bn) * 128 B at the ~80 B/clk an SM sustains from L2 (profiles/r01b_ncu_gemm1_ffn2.txt: 80.7 B/clk with the
-// tensor pipe at 85 %) takes 1.6 * (128 + bn); a shape costs waves * max of the two.
+// Cost model of one 128 x bn tile over one 64-wide k-block, in SM clocks: the MMA takes 4*bn at the H100 SXM
+// data-sheet rate (989 TFLOP/s dense bf16 over 132 SMs at 1.83 GHz = 4096 FLOP/clk), the operand fetch
+// (128 + bn) * 128 B at an assumed 64 B/clk per SM from L2; a shape costs waves * max of the two.
 static double flex_tile_cost(int bn) {
-  const double mma = 2.0 * bn, fetch = 1.6 * (128 + bn);
+  const double mma = 4.0 * bn, fetch = 2.0 * (128 + bn);
   return mma > fetch ? mma : fetch;
 }
 // Best runtime tile width for a shape the fixed-width kernels fill badly, or 0 to keep them.
@@ -447,32 +205,28 @@ int gemm_flex_bn(int epi, int M, int N, int K) {
   return best;
 }
 
-template <bool kBf16, int kEpi>
-static int launch_flex(const void* a, int lda, const void* w, int ldw, const GemmParams& p, int bn,
-                       cudaStream_t stream) {
+template <int BN, bool kBf16, int kEpi>
+static int launch_flex(const void* a, int lda, const void* w, int ldw, const GemmParams& p, cudaStream_t stream) {
+  using Cfg = GemmCfg<BN>;
   CUtensorMap ta, tb;
   int rc = make_tmap_2d(&ta, a, p.M, p.K, lda, BLOCK_M, BLOCK_K, kBf16);
   if (rc != KR_OK) return rc;
-  rc = make_tmap_2d(&tb, w, p.N, p.K, ldw, bn, BLOCK_K, kBf16);
+  rc = make_tmap_2d(&tb, w, p.N, p.K, ldw, BN, BLOCK_K, kBf16);
   if (rc != KR_OK) return rc;
-  const int stage_bytes = BLOCK_M * BLOCK_K * 2 + bn * BLOCK_K * 2;
-  int stages = (200 * 1024) / stage_bytes;
-  if (stages > 8) stages = 8;
-  const int smem = stages * stage_bytes + 1024 + 256;
-  auto kern = gemm_flex_kernel<kBf16, kEpi>;
+  auto kern = gemm_flex_kernel<BN, kBf16, kEpi>;
   static bool attr_set = false;
   if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 208 * 1024);
+    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes);
     if (e != cudaSuccess) {
       set_last_error("gemm_flex: cudaFuncSetAttribute failed: %s", cudaGetErrorString(e));
       return KR_ERR_CUDA;
     }
     attr_set = true;
   }
-  const int num_tiles = ((p.M + BLOCK_M - 1) / BLOCK_M) * ((p.N + bn - 1) / bn);
+  const int num_tiles = ((p.M + BLOCK_M - 1) / BLOCK_M) * ((p.N + BN - 1) / BN);
   int grid = sm_count();
   if (grid > num_tiles) grid = num_tiles;
-  kern<<<grid, kNumThreads, smem, stream>>>(ta, tb, p, bn, stages);
+  kern<<<grid, kNumThreads, Cfg::kSmemBytes, stream>>>(ta, tb, p);
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) {
     set_last_error("gemm_flex: launch failed: %s", cudaGetErrorString(e));
@@ -481,10 +235,23 @@ static int launch_flex(const void* a, int lda, const void* w, int ldw, const Gem
   return KR_OK;
 }
 
+template <bool kBf16, int kEpi>
+static int flex_width(const void* a, int lda, const void* w, int ldw, const GemmParams& p, int bn, cudaStream_t s) {
+  switch (bn) {
+    case 96: return launch_flex<96, kBf16, kEpi>(a, lda, w, ldw, p, s);
+    case 128: return launch_flex<128, kBf16, kEpi>(a, lda, w, ldw, p, s);
+    case 160: return launch_flex<160, kBf16, kEpi>(a, lda, w, ldw, p, s);
+    case 192: return launch_flex<192, kBf16, kEpi>(a, lda, w, ldw, p, s);
+    case 224: return launch_flex<224, kBf16, kEpi>(a, lda, w, ldw, p, s);
+    case 256: return launch_flex<256, kBf16, kEpi>(a, lda, w, ldw, p, s);
+    default: set_last_error("gemm_flex: unsupported tile width %d", bn); return KR_ERR_INVALID_ARG;
+  }
+}
+
 static int gemm_flex(int dtype, int epi, const void* a, int lda, const void* w, int ldw, const GemmParams& p, int bn,
                      cudaStream_t s) {
   const bool bf = dtype == 0;
-#define KR_FLEX(E) (bf ? launch_flex<true, E>(a, lda, w, ldw, p, bn, s) : launch_flex<false, E>(a, lda, w, ldw, p, bn, s))
+#define KR_FLEX(E) (bf ? flex_width<true, E>(a, lda, w, ldw, p, bn, s) : flex_width<false, E>(a, lda, w, ldw, p, bn, s))
   switch (epi) {
     case EPI_BIAS: return KR_FLEX(EPI_BIAS);
     case EPI_BIAS_GELU: return KR_FLEX(EPI_BIAS_GELU);
@@ -512,43 +279,32 @@ static int dispatch_epi(int epi, const void* a, int lda, const void* w, int ldw,
 }
 
 // dtype: 0 = bf16, 1 = fp16
-// Which kernel serves a shape.  Costs are per-SM tile-times in units of one CTA-pair tile (a single-CTA
-// 128x256 tile is the same work per SM but runs at ~0.88 instead of ~0.98 of the tensor peak -> 1.12):
-//   0  the single-CTA kernel below                  ceil(tiles128 / SMs) * 1.12
-//   1  the CTA-pair kernel (kr_gemm2.cu)            ceil(tiles256 / pairs)
-// M = 4680: N = 15360 -> 16 vs 16.8, N = 13824 -> 14 vs 15.7 (pair); N = 5120 -> 6 vs 5.6 (single CTA: 380
-// pair tiles are 5.14 waves of 74 pairs).  A hybrid plan (pair kernel on the first 4608 rows, single-CTA
-// kernel on the last 72 rows on a side stream so its 20 tiles fill the SMs the pair kernel's partial last
-// wave leaves idle; predicted 5.1) was built and measured: 1406 vs 1426 TF/s on ffn.2, 1491 vs 1505 on
-// to_qkv, 16.21 / 16.12 vs 16.23 / 16.26 fps in same-box bench runs -> not kept
-// (profiles/r01_gemm_hybrid_plan_*.log).
-// KR_GEMM2: 0 = never the pair kernel, 1 = by cost (default), 2 = pair whenever N % 256 == 0 (tests)
+// Which kernel serves a shape:
+//   0  the fixed-width kernel above
+//   1  the 2-CTA cluster kernel (kr_gemm2.cu): same work per SM per wave as two 128x256 tiles, half the W traffic.
+//      Measured on an H100 SXM (400 W limit, bench shapes M = 4680): 275 TFLOP/s against 446 for the single-CTA
+//      kernel (its consumers hold a stage until both CTAs release it), so a pair-tile wave is costed 1.62 single
+//      waves and the bench shapes keep the single-CTA kernels
+//   2  stream-K (kr_gemm_sk.cu), only with a workspace and KR_GEMM_SK=1, when the data-parallel wave efficiency is poor
+//   3  the runtime-width kernel (gemm_flex_bn)
+// KR_GEMM2: 0 = never the cluster kernel, 1 = by the wave count (default), 2 = whenever N % 256 == 0 (tests)
 int gemm_plan(int epi, int M, int N, int K, bool have_workspace) {
   static const int mode = [] { const char* e = getenv("KR_GEMM2"); return e != nullptr ? atoi(e) : 1; }();
-  // KR_GEMM_SK: 0 = never stream-K (default until it beats the data-parallel kernels: profiles/r02_gemm_ab.log),
-  // 1 = when the data-parallel wave efficiency is poor
+  // KR_GEMM_SK: 0 = never stream-K (default), 1 = when the data-parallel wave efficiency is poor
   static const int sk_mode = [] { const char* e = getenv("KR_GEMM_SK"); return e != nullptr ? atoi(e) : 0; }();
-  if (have_workspace && sk_mode > 0 && gemm_sk_preferred(epi, M, N, K)) {
-    // the CTA-pair kernel keeps shapes it fills well (its tiles are twice as large): pair waves vs stream-K
-    const int sms_ = sm_count(), pairs_ = sms_ / 2;
-    const long tp = static_cast<long>((M + 255) / 256) * (N / 256);
-    const double pair_eff = (mode > 0 && N % 256 == 0 && tp >= 4L * pairs_)
-        ? static_cast<double>(M) / 256.0 * (N / 256) / static_cast<double>(((tp + pairs_ - 1) / pairs_) * pairs_) : 0.0;
-    if (pair_eff < 0.80) return 2;
-  }
+  if (have_workspace && sk_mode > 0 && gemm_sk_preferred(epi, M, N, K)) return 2;
   const int flex = (epi == EPI_F32) ? 0 : gemm_flex_bn(epi, M, N, K);
   if (mode <= 0 || epi == EPI_F32 || epi == EPI_MUL || N % 256 != 0 || K < 256) return flex ? 3 : 0;
   if (mode == 2) return 1;
   const int sms = sm_count(), pairs = sms / 2, nb = N / 256;
   const long tiles1 = static_cast<long>((M + 127) / 128) * nb;
-  const double cost1 = static_cast<double>((tiles1 + sms - 1) / sms) * 1.12;
-  const long tiles_f = static_cast<long>((M + 255) / 256) * nb;
-  if (tiles_f < 4L * pairs) return flex ? 3 : 0;
-  const double cost_f = static_cast<double>((tiles_f + pairs - 1) / pairs);
-  if (cost_f < cost1) return 1;
+  const long tiles_p = static_cast<long>((M + 255) / 256) * nb;
+  if (tiles_p < 4L * pairs) return flex ? 3 : 0;
+  constexpr double kPairWaveCost = 1.62;   // measured cluster vs single-CTA tile throughput, see above
+  if (static_cast<double>((tiles_p + pairs - 1) / pairs) * kPairWaveCost <= static_cast<double>((tiles1 + sms - 1) / sms))
+    return 1;
   return flex ? 3 : 0;
 }
-bool gemm_uses_pair(int epi, int M, int N, int K) { return gemm_plan(epi, M, N, K) == 1; }
 
 namespace {
 int gemm_single(int dtype, int epi, const void* a, int lda, const void* w, int ldw, const GemmParams& p,

@@ -1,177 +1,32 @@
-// kr_gemm2.cu — 2-CTA (cta_group::2) variant of the persistent tcgen05 GEMM.
+// kr_gemm2.cu — 2-CTA cluster variant of the persistent wgmma GEMM (kr_gemm.cu) for the wide DiT projections.
 //
-// Same contract as kr_gemm.cu (C = epilogue(A W^T + bias), K-major 16-bit operands) for the two
-// widest projections of the DiT block (to_qkv N=15360, ffn.0 N=13824), where the single-CTA kernel
-// is limited by shared-memory / L2->SM operand traffic (48 KB per 128x256x64 k-block per SM).
-// A CTA PAIR (cluster of 2 on one TPC) computes a 256x256 tile with ONE tcgen05.mma.cta_group::2
-// (M=256, N=256, K=16) per k-step: each CTA stages its own 128 rows of A and HALF of the W tile
-// (128 rows), the tensor cores of both SMs read both halves -> 32 KB per k-block per SM.
-//   warp 0 (both CTAs) : TMA producer; loads signal the LEADER's full barrier (cta_group::2)
-//   warp 1 (leader)    : issues the MMAs; commits with multicast to both CTAs' barriers
-//   warps 2..5 (both)  : epilogue of the CTA's own 128 rows out of its own TMEM
-// Barriers: full[stage] on the leader (expects the bytes of both CTAs); empty[stage] and
-// tmem_full[acc] in each CTA (arrived by the leader's multicast commit); tmem_empty[acc] on the
-// leader (4 epilogue warps x 2 CTAs, the peer arrives remotely).
+//   C[M,N] = epilogue( A[M,K] @ W[N,K]^T + bias[N] )        same operands / epilogues as kr_gemm.cu
+//
+// The two CTAs of a cluster compute the vertically adjacent 128 x 256 tiles (m, n) and (m+1, n), which use the
+// same 256 x 64 W block per k-block.  Each CTA loads its own A tile and HALF of that W block, multicast into both
+// CTAs (TMA .multicast::cluster), so the W operand crosses L2 -> SM once per pair of tiles instead of twice: a
+// stage costs each SM 16 KB of A + 16 KB of W instead of 16 + 32 KB.
+// Pipeline: a stage's full barrier expects A + the whole W block (both halves signal it); its empty barrier
+// collects one arrive from each consumer warpgroup of BOTH CTAs (remote arrives through mapa), because the peer
+// overwrites this CTA's W half when it refills the stage.  Roles are those of kr_gemm.cu: consumer warpgroups
+// 0, 1 (64 rows each), TMA warpgroup 2.
 #include "kr_common.cuh"
+#include "kr_gemm_epi.cuh"
 #include "kr_ops.h"
+
+#include <cstdlib>
 
 namespace kr {
 
-static constexpr int G2_BLOCK_M = 128;          // rows per CTA (256 per pair)
-static constexpr int G2_BLOCK_N = 256;
-static constexpr int G2_BLOCK_K = 128;         // two 64-element SWIZZLE_128B panels per operand per stage
-static constexpr int G2_THREADS = 192;
-static constexpr int G2_PANEL = G2_BLOCK_M * 64 * 2;                    // 16 KB: 128 rows x 64 elements
-static constexpr int G2_A_BYTES = 2 * G2_PANEL;                         // 32 KB
-static constexpr int G2_B_BYTES = 2 * G2_PANEL;                         // 32 KB (half of the W tile: 128 rows)
-static constexpr int G2_STAGE_BYTES = G2_A_BYTES + G2_B_BYTES;
-static constexpr int G2_STAGES = 3;
-static constexpr int G2_SMEM = G2_STAGES * G2_STAGE_BYTES + 1024 + 256;
-
-KR_DEVICE uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-KR_DEVICE void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-  asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-// TMA load whose completion bytes are credited to the LEADER CTA's mbarrier (same smem offset)
-KR_DEVICE void tma_load_2d_pair(void* smem_dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1) {
-  const uint32_t bar_leader = smem_u32(bar) & 0xFEFFFFFFu;     // clear the peer bit -> CTA rank 0
-  asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes"
-      " [%0], [%1, {%3, %4}], [%2];" ::"r"(smem_u32(smem_dst)),
-      "l"(reinterpret_cast<uint64_t>(m)), "r"(bar_leader), "r"(c0), "r"(c1)
-      : "memory");
-}
-KR_DEVICE void umma_ss_pair(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc,
-                            uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t"
-      "}\n" ::"r"(d_tmem),
-      "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// arrive (once the issued MMAs retire) on the barrier at this smem offset in BOTH CTAs of the pair
-KR_DEVICE void umma_commit_pair(uint64_t* bar) {
-  const uint16_t mask = 3;
-  asm volatile(
-      "tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(
-          smem_u32(bar)),
-      "h"(mask)
-      : "memory");
-}
-KR_DEVICE void mbar_arrive_on_leader(uint64_t* bar) {
-  asm volatile(
-      "{\n\t"
-      ".reg .b32 ra;\n\t"
-      "mapa.shared::cluster.u32 ra, %0, 0;\n\t"
-      "mbarrier.arrive.shared::cluster.b64 _, [ra];\n\t"
-      "}\n" ::"r"(smem_u32(bar))
-      : "memory");
-}
-template <uint32_t kCols>
-KR_DEVICE void tmem_alloc_pair(uint32_t* smem_result) {
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(
-                   smem_u32(smem_result)),
-               "n"(kCols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-template <uint32_t kCols>
-KR_DEVICE void tmem_dealloc_pair(uint32_t taddr) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "n"(kCols)
-               : "memory");
-}
-
-// one 32-column chunk of the fused epilogue (same arithmetic / rounding points as kr_gemm.cu)
-template <bool kBf16, int kEpi>
-KR_DEVICE void epilogue_chunk(const GemmParams& p, const uint32_t (&r)[32], int row, int col0,
-                              const uint16_t* gate_row) {
-  float v[32];
-#pragma unroll
-  for (int j = 0; j < 32; ++j) v[j] = __uint_as_float(r[j]);
-  auto unpack = [](uint32_t u) -> float2 { return kBf16 ? unpack_bf16x2(u) : unpack_f16x2(u); };
-  auto rnd = [](float x) -> float {
-    return kBf16 ? __bfloat162float(__float2bfloat16_rn(x)) : __half2float(__float2half_rn(x));
-  };
-  if (p.bias != nullptr) {
-    const uint4* b4 = reinterpret_cast<const uint4*>(reinterpret_cast<const uint16_t*>(p.bias) + col0);
-#pragma unroll
-    for (int q = 0; q < 4; ++q) {
-      const uint4 bb = __ldg(b4 + q);
-      const uint32_t w[4] = {bb.x, bb.y, bb.z, bb.w};
-#pragma unroll
-      for (int h = 0; h < 4; ++h) {
-        const float2 f = unpack(w[h]);
-        v[q * 8 + h * 2] += f.x;
-        v[q * 8 + h * 2 + 1] += f.y;
-      }
-    }
-  }
-  if constexpr (kEpi == EPI_BIAS_GELU) {
-#pragma unroll
-    for (int j = 0; j < 32; ++j) v[j] = gelu_tanh(rnd(v[j]));
-  }
-  if constexpr (kEpi == EPI_BIAS_GATE_RES) {
-    const uint4* g4 = reinterpret_cast<const uint4*>(gate_row + col0);
-#pragma unroll
-    for (int q = 0; q < 4; ++q) {
-      const uint4 gg = __ldg(g4 + q);
-      const uint32_t w[4] = {gg.x, gg.y, gg.z, gg.w};
-#pragma unroll
-      for (int h = 0; h < 4; ++h) {
-        const float2 f = unpack(w[h]);
-        v[q * 8 + h * 2] = rnd(rnd(v[q * 8 + h * 2]) * f.x);
-        v[q * 8 + h * 2 + 1] = rnd(rnd(v[q * 8 + h * 2 + 1]) * f.y);
-      }
-    }
-  }
-  if constexpr (kEpi == EPI_BIAS_GATE_RES || kEpi == EPI_BIAS_RES) {
-    const uint4* r4 = reinterpret_cast<const uint4*>(
-        reinterpret_cast<const uint16_t*>(p.residual) + static_cast<size_t>(row) * p.ldr + col0);
-#pragma unroll
-    for (int q = 0; q < 4; ++q) {
-      const uint4 rr = r4[q];
-      const uint32_t w[4] = {rr.x, rr.y, rr.z, rr.w};
-#pragma unroll
-      for (int h = 0; h < 4; ++h) {
-        const float2 f = unpack(w[h]);
-        if constexpr (kEpi == EPI_BIAS_RES) {
-          v[q * 8 + h * 2] = f.x + rnd(v[q * 8 + h * 2]);
-          v[q * 8 + h * 2 + 1] = f.y + rnd(v[q * 8 + h * 2 + 1]);
-        } else {
-          v[q * 8 + h * 2] = f.x + v[q * 8 + h * 2];
-          v[q * 8 + h * 2 + 1] = f.y + v[q * 8 + h * 2 + 1];
-        }
-      }
-    }
-  }
-  uint16_t* o = (p.out2 != nullptr && col0 >= p.n_split)
-      ? reinterpret_cast<uint16_t*>(p.out2) + static_cast<size_t>(row) * p.ldc2 + (col0 - p.n_split)
-      : reinterpret_cast<uint16_t*>(p.out) + static_cast<size_t>(row) * p.ldc + col0;
-#pragma unroll
-  for (int q = 0; q < 4; ++q) {
-    uint4 w;
-    if (kBf16) {
-      w.x = pack_bf16x2(v[q * 8 + 0], v[q * 8 + 1]);
-      w.y = pack_bf16x2(v[q * 8 + 2], v[q * 8 + 3]);
-      w.z = pack_bf16x2(v[q * 8 + 4], v[q * 8 + 5]);
-      w.w = pack_bf16x2(v[q * 8 + 6], v[q * 8 + 7]);
-    } else {
-      w.x = pack_f16x2(v[q * 8 + 0], v[q * 8 + 1]);
-      w.y = pack_f16x2(v[q * 8 + 2], v[q * 8 + 3]);
-      w.z = pack_f16x2(v[q * 8 + 4], v[q * 8 + 5]);
-      w.w = pack_f16x2(v[q * 8 + 6], v[q * 8 + 7]);
-    }
-    reinterpret_cast<uint4*>(o)[q] = w;
-  }
-}
+namespace {
+constexpr int G2_BM = 128, G2_BN = 256, G2_BK = 64;
+constexpr int G2_THREADS = 384;
+constexpr int G2_STAGES = 4;
+constexpr int G2_A_BYTES = G2_BM * G2_BK * 2, G2_B_BYTES = G2_BN * G2_BK * 2;
+constexpr int G2_STAGE_BYTES = G2_A_BYTES + G2_B_BYTES;
+constexpr int G2_SCR_BYTES = 8 * kEpiScrFloats * 4;
+constexpr int G2_SMEM = G2_STAGES * G2_STAGE_BYTES + G2_SCR_BYTES + 1024 + 256;
+}  // namespace
 
 template <bool kBf16, int kEpi>
 __global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(G2_THREADS, 1)
@@ -182,169 +37,76 @@ gemm2_tn_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constan
                                              ~static_cast<uintptr_t>(1023));
   uint8_t* smem_a = smem;
   uint8_t* smem_b = smem + G2_STAGES * G2_A_BYTES;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + G2_STAGES * G2_STAGE_BYTES);
-  uint64_t* full_bar = bars;                     // [stages]  (used on the leader)
-  uint64_t* empty_bar = bars + G2_STAGES;        // [stages]  (per CTA)
-  uint64_t* tmem_full = bars + 2 * G2_STAGES;    // [2]       (per CTA)
-  uint64_t* tmem_empty = tmem_full + 2;          // [2]       (used on the leader)
-  uint32_t* tmem_base_smem = reinterpret_cast<uint32_t*>(tmem_empty + 2);
+  float* scratch = reinterpret_cast<float*>(smem + G2_STAGES * G2_STAGE_BYTES);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + G2_STAGES * G2_STAGE_BYTES + G2_SCR_BYTES);
+  uint64_t* full_bar = bars;
+  uint64_t* empty_bar = bars + G2_STAGES;
 
   const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
-  const uint32_t cta_rank = cluster_ctarank();
-  const bool leader = cta_rank == 0;
-  const int pair = blockIdx.x >> 1;
-  const int num_pairs = gridDim.x >> 1;
+  const uint32_t rank = cluster_ctarank();
+  const int num_m = (p.M + G2_BM - 1) / G2_BM;
+  const int num_pm = (num_m + 1) / 2;                 // row-block pairs (the last CTA of an odd count computes zeros)
+  const int num_n = p.N / G2_BN;
+  const int num_pairs = num_pm * num_n;
+  const int num_k = (p.K + G2_BK - 1) / G2_BK;
+  const int cluster = blockIdx.x >> 1, num_clusters = gridDim.x >> 1;
 
-  const int num_m = (p.M + 2 * G2_BLOCK_M - 1) / (2 * G2_BLOCK_M);
-  const int num_n = p.N / G2_BLOCK_N;
-  const int num_tiles = num_m * num_n;
-  const int num_k = (p.K + G2_BLOCK_K - 1) / G2_BLOCK_K;
-
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 256) {
     prefetch_tmap(&tmap_a);
     prefetch_tmap(&tmap_b);
-  }
-  if (warp == 1) {
-    if (lane == 0) {
-      for (int i = 0; i < G2_STAGES; ++i) {
-        mbar_init(&full_bar[i], 1);
-        mbar_init(&empty_bar[i], 1);
-      }
-      for (int i = 0; i < 2; ++i) {
-        mbar_init(&tmem_full[i], 1);
-        mbar_init(&tmem_empty[i], 8);      // 4 epilogue warps x 2 CTAs
-      }
-      fence_barrier_init();
+    for (int i = 0; i < G2_STAGES; ++i) {
+      mbar_init(&full_bar[i], 1);
+      mbar_init(&empty_bar[i], 4);   // 2 consumer warpgroups x 2 CTAs
     }
-    __syncwarp();
-    tmem_alloc_pair<512>(tmem_base_smem);
+    fence_barrier_init();
   }
-  tc_fence_before();
-  __syncthreads();
-  cluster_sync_all();                      // peer barriers initialised before any remote signal
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_base_smem;
+  cluster_sync();
 
-  if (warp == 0) {
-    // ===================== TMA producer (both CTAs) =====================
-    if (elect_one()) {
+  if (warp >= 8) {
+    producer_regs();
+    if (warp == 8 && elect_one()) {
       int stage = 0;
       uint32_t phase = 0;
-      for (int tile = pair; tile < num_tiles; tile += num_pairs) {
-        const int m_blk = tile % num_m;
-        const int n_blk = tile / num_m;
-        const int row0 = m_blk * 2 * G2_BLOCK_M + cta_rank * G2_BLOCK_M;          // my A rows
-        const int wrow0 = n_blk * G2_BLOCK_N + cta_rank * (G2_BLOCK_N / 2);      // my half of W rows
+      for (int t = cluster; t < num_pairs; t += num_clusters) {
+        const int m_blk = 2 * (t % num_pm) + static_cast<int>(rank), n_blk = t / num_pm;
         for (int kb = 0; kb < num_k; ++kb) {
           mbar_wait(&empty_bar[stage], phase ^ 1);
-          if (leader) mbar_expect_tx(&full_bar[stage], 2 * G2_STAGE_BYTES);      // bytes of both CTAs
-#pragma unroll
-          for (int h = 0; h < 2; ++h) {
-            tma_load_2d_pair(smem_a + stage * G2_A_BYTES + h * G2_PANEL, &tmap_a, &full_bar[stage],
-                             kb * G2_BLOCK_K + h * 64, row0);
-            tma_load_2d_pair(smem_b + stage * G2_B_BYTES + h * G2_PANEL, &tmap_b, &full_bar[stage],
-                             kb * G2_BLOCK_K + h * 64, wrow0);
-          }
+          mbar_expect_tx(&full_bar[stage], G2_STAGE_BYTES);
+          tma_load_2d(smem_a + stage * G2_A_BYTES, &tmap_a, &full_bar[stage], kb * G2_BK, m_blk * G2_BM);
+          tma_load_2d_mc(smem_b + stage * G2_B_BYTES + rank * (G2_B_BYTES / 2), &tmap_b, &full_bar[stage],
+                         kb * G2_BK, n_blk * G2_BN + static_cast<int>(rank) * (G2_BN / 2), 0x3);
           if (++stage == G2_STAGES) {
             stage = 0;
             phase ^= 1;
           }
-        }
-      }
-    }
-  } else if (warp == 1) {
-    // ===================== MMA issuer (leader CTA only, ONE thread runs the whole loop) =====================
-    if (leader && elect_one()) {
-      constexpr uint32_t idesc = make_idesc<kBf16>(2 * G2_BLOCK_M, G2_BLOCK_N, 0, 0);
-      // descriptor = constant high word | (start address >> 4); K-major SW128: LBO 16 B, SBO 1024 B
-      const uint64_t desc_hi = make_smem_desc(0, 16, 1024) & 0xFFFFFFFF00000000ull;
-      const uint32_t desc_lo_c = static_cast<uint32_t>(make_smem_desc(0, 16, 1024));
-      const uint32_t a0 = smem_u32(smem_a), b0 = smem_u32(smem_b);
-      int stage = 0;
-      uint32_t phase = 0;
-      int acc = 0;
-      uint32_t acc_phase = 0;
-      for (int tile = pair; tile < num_tiles; tile += num_pairs) {
-        mbar_wait(&tmem_empty[acc], acc_phase ^ 1);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + acc * G2_BLOCK_N;
-        for (int kb = 0; kb < num_k; ++kb) {
-          mbar_wait(&full_bar[stage], phase);
-          tc_fence_after();
-          const uint32_t a_lo = desc_lo_c | (((a0 + stage * G2_A_BYTES) & 0x3FFFF) >> 4);
-          const uint32_t b_lo = desc_lo_c | (((b0 + stage * G2_B_BYTES) & 0x3FFFF) >> 4);
-#pragma unroll
-          for (int k = 0; k < G2_BLOCK_K / 16; ++k) {
-            const uint32_t off = ((k >> 2) * G2_PANEL + (k & 3) * 32) >> 4;
-            umma_ss_pair(d_tmem, desc_hi | (a_lo + off), desc_hi | (b_lo + off), idesc, (kb | k) != 0 ? 1u : 0u);
-          }
-          umma_commit_pair(&empty_bar[stage]);
-          if (kb == num_k - 1) umma_commit_pair(&tmem_full[acc]);
-          if (++stage == G2_STAGES) {
-            stage = 0;
-            phase ^= 1;
-          }
-        }
-        if (++acc == 2) {
-          acc = 0;
-          acc_phase ^= 1;
         }
       }
     }
   } else {
-    // ===================== epilogue warps (both CTAs, own 128 rows) =====================
-    const int quarter = warp & 3;
-    int acc = 0;
-    uint32_t acc_phase = 0;
-    for (int tile = pair; tile < num_tiles; tile += num_pairs) {
-      const int m_blk = tile % num_m;
-      const int n_blk = tile / num_m;
-      const int row = m_blk * 2 * G2_BLOCK_M + cta_rank * G2_BLOCK_M + quarter * 32 + lane;
-      const bool row_ok = row < p.M;
-      mbar_wait(&tmem_full[acc], acc_phase);
-      tc_fence_after();
-      const uint32_t t_row = tmem_base + (static_cast<uint32_t>(quarter * 32) << 16) + acc * G2_BLOCK_N;
-      const uint16_t* gate_row = nullptr;
-      if constexpr (kEpi == EPI_BIAS_GATE_RES) {
-        const int g = row_ok ? (row + p.row_offset) / p.rows_per_gate : 0;
-        gate_row = reinterpret_cast<const uint16_t*>(p.gate) + static_cast<size_t>(g) * p.gate_stride;
-      }
-#pragma unroll 1
-      for (int c = 0; c < G2_BLOCK_N / 32; ++c) {
-        uint32_t r[32];
-        tmem_ld_x32(t_row + c * 32, r);
-        tmem_ld_wait();
-        if (c == G2_BLOCK_N / 32 - 1) {
-          tc_fence_before();
-          __syncwarp();
-          if (lane == 0) mbar_arrive_on_leader(&tmem_empty[acc]);
-        }
-        if (row_ok) epilogue_chunk<kBf16, kEpi>(p, r, row, n_blk * G2_BLOCK_N + c * 32, gate_row);
-      }
-      if (++acc == 2) {
-        acc = 0;
-        acc_phase ^= 1;
-      }
+    consumer_regs();
+    const int wg = warp >> 2;
+    const uint32_t a_base = smem_u32(smem_a) + wg * 64 * 128, b_base = smem_u32(smem_b);
+    float* scr = scratch + warp * kEpiScrFloats;
+    int stage = 0;
+    uint32_t phase = 0;
+    for (int t = cluster; t < num_pairs; t += num_clusters) {
+      const int m_blk = 2 * (t % num_pm) + static_cast<int>(rank), n_blk = t / num_pm;
+      float acc[G2_BN / 2];
+      gemm_mainloop<G2_BN, kBf16 ? 0 : 1, 2>(acc, a_base, b_base, G2_A_BYTES, G2_B_BYTES, G2_STAGES, full_bar,
+                                             empty_bar, stage, phase, 0, num_k);
+      gemm_frag_epilogue<G2_BN, kBf16, kEpi>(acc, scr, m_blk * G2_BM + wg * 64 + (warp & 3) * 16, n_blk * G2_BN,
+                                             G2_BN, 1.0f, p);
     }
   }
-
-  tc_fence_before();
-  __syncthreads();
-  cluster_sync_all();                      // nobody leaves (or frees TMEM) while the pair still works
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc_pair<512>(tmem_base);
-  }
+  cluster_sync();
 }
 
 template <bool kBf16, int kEpi>
-static int launch_gemm2(const void* a, int lda, const void* w, int ldw, const GemmParams& p,
-                        cudaStream_t stream) {
+static int launch_gemm2(const void* a, int lda, const void* w, int ldw, const GemmParams& p, cudaStream_t stream) {
   CUtensorMap ta, tb;
-  int rc = make_tmap_2d(&ta, a, p.M, p.K, lda, G2_BLOCK_M, 64, kBf16);
+  int rc = make_tmap_2d(&ta, a, p.M, p.K, lda, G2_BM, G2_BK, kBf16);
   if (rc != KR_OK) return rc;
-  rc = make_tmap_2d(&tb, w, p.N, p.K, ldw, G2_BLOCK_N / 2, 64, kBf16);
+  rc = make_tmap_2d(&tb, w, p.N, p.K, ldw, G2_BN / 2, G2_BK, kBf16);
   if (rc != KR_OK) return rc;
   auto kern = gemm2_tn_kernel<kBf16, kEpi>;
   static bool attr_set = false;
@@ -356,10 +118,10 @@ static int launch_gemm2(const void* a, int lda, const void* w, int ldw, const Ge
     }
     attr_set = true;
   }
-  const int num_tiles = ((p.M + 2 * G2_BLOCK_M - 1) / (2 * G2_BLOCK_M)) * (p.N / G2_BLOCK_N);
-  int pairs = sm_count() / 2;
-  if (pairs > num_tiles) pairs = num_tiles;
-  kern<<<2 * pairs, G2_THREADS, G2_SMEM, stream>>>(ta, tb, p);
+  const int pairs = ((p.M + G2_BM - 1) / G2_BM + 1) / 2 * (p.N / G2_BN);
+  int clusters = sm_count() / 2;
+  if (clusters > pairs) clusters = pairs;
+  kern<<<2 * clusters, G2_THREADS, G2_SMEM, stream>>>(ta, tb, p);
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) {
     set_last_error("gemm2: launch failed: %s", cudaGetErrorString(e));
@@ -368,21 +130,19 @@ static int launch_gemm2(const void* a, int lda, const void* w, int ldw, const Ge
   return KR_OK;
 }
 
+// N % 256 == 0 (the planner only sends such shapes here)
 int gemm2_tn(int dtype, int epi, const void* a, int lda, const void* w, int ldw, const GemmParams& p,
              cudaStream_t stream) {
   const bool bf = dtype == 0;
-#define KR_G2_CASE(E) \
-  case E: return bf ? launch_gemm2<true, E>(a, lda, w, ldw, p, stream) : launch_gemm2<false, E>(a, lda, w, ldw, p, stream);
+#define KR_G2(E) (bf ? launch_gemm2<true, E>(a, lda, w, ldw, p, stream) : launch_gemm2<false, E>(a, lda, w, ldw, p, stream))
   switch (epi) {
-    KR_G2_CASE(EPI_BIAS)
-    KR_G2_CASE(EPI_BIAS_GELU)
-    KR_G2_CASE(EPI_BIAS_GATE_RES)
-    KR_G2_CASE(EPI_BIAS_RES)
-    default:
-      set_last_error("gemm2: epilogue %d not supported by the CTA-pair kernel", epi);
-      return KR_ERR_INVALID_ARG;
+    case EPI_BIAS: return KR_G2(EPI_BIAS);
+    case EPI_BIAS_GELU: return KR_G2(EPI_BIAS_GELU);
+    case EPI_BIAS_GATE_RES: return KR_G2(EPI_BIAS_GATE_RES);
+    case EPI_BIAS_RES: return KR_G2(EPI_BIAS_RES);
+    default: set_last_error("gemm2: unsupported epilogue %d", epi); return KR_ERR_INVALID_ARG;
   }
-#undef KR_G2_CASE
+#undef KR_G2
 }
 
 }  // namespace kr

@@ -1,4 +1,4 @@
-// kr_gemm_fp8.cu — FP8 (e4m3) tcgen05 GEMM with per-tensor scales + the dynamic activation quantisation kernels.
+// kr_gemm_fp8.cu — FP8 (e4m3) wgmma GEMM with per-tensor scales + the dynamic activation quantisation kernels.
 //
 //   out[M,N] = epilogue( (Aq[M,K] @ Wq[N,K]^T) * scale_a * scale_w + bias[N] )      Aq, Wq e4m3, out bf16
 //
@@ -6,13 +6,13 @@
 // granularity=PerTensor()))` (release_server.py:179-182, `enable_fp8: true`) turns every nn.Linear into: torchao's
 // dynamic per-tensor activation cast (amax over the whole activation -> scale = 448 / amax -> saturating e4m3 cast)
 // followed by torch._scaled_mm (cuBLASLt FP8, fp32 accumulation, bf16 output) — here a hand-written
-// tcgen05.mma.kind::f8f6f4 kernel with the same fused epilogues as the bf16 GEMM (bias, GELU, gate + residual, ...).
+// wgmma e4m3 kernel with the same fused epilogues as the bf16 GEMM (bias, GELU, gate + residual, ...).
 // torchao is absent from the image: the algorithm is restated from its published definition (oracle/fp8_oracle.py).
 //
-// Kernel structure = kr_gemm.cu (persistent 1 CTA/SM, TMA producer warp, one elected MMA thread, 4 epilogue warps,
-// TMEM accumulators double-buffered), with byte-sized elements: a 128-byte swizzle row holds 128 k-elements, one
-// MMA consumes K = 32 (32 bytes), so a 48 KB stage (A 128x128 B, W 256x128 B) feeds 4 MMAs of 128 clk — twice the
-// FLOPs of the bf16 kernel per byte moved.
+// Kernel structure = kr_gemm.cu (persistent 1 CTA/SM, two consumer warpgroups with register accumulators, a TMA
+// warpgroup), with byte-sized elements: a 128-byte swizzle row holds 128 k-elements, one wgmma consumes K = 32
+// (32 bytes); each 128-wide k-block is accumulated separately and added to the fp32 registers (the e4m3 wgmma
+// adder keeps fewer mantissa bits), so the tile is 128 x 128 to leave registers for the partial.
 #include "kr_common.cuh"
 #include "kr_gemm_epi.cuh"
 #include "kr_ops.h"
@@ -22,21 +22,11 @@
 namespace kr {
 
 namespace {
-constexpr int F8_BM = 128, F8_BN = 256, F8_BK = 128 /* elements = bytes */, F8_UK = 32;
-constexpr int F8_THREADS = 192, F8_STAGES = 4;
+constexpr int F8_BM = 128, F8_BN = 128, F8_BK = 128 /* elements = bytes */;
+constexpr int F8_THREADS = 384, F8_STAGES = 4;
 constexpr int F8_A_BYTES = F8_BM * F8_BK, F8_B_BYTES = F8_BN * F8_BK, F8_STAGE_BYTES = F8_A_BYTES + F8_B_BYTES;
-constexpr int F8_SMEM = F8_STAGES * F8_STAGE_BYTES + 1024 + 256;
-
-KR_DEVICE void umma_ss_f8(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f8f6f4 [%0], %1, %2, %3, p;\n\t"
-      "}\n" ::"r"(d_tmem),
-      "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
+constexpr int F8_SCR_BYTES = 8 * kEpiScrFloats * 4;
+constexpr int F8_SMEM = F8_STAGES * F8_STAGE_BYTES + F8_SCR_BYTES + 1024 + 256;
 }  // namespace
 
 template <int kEpi>
@@ -48,44 +38,29 @@ gemm_fp8_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constan
                                              ~static_cast<uintptr_t>(1023));
   uint8_t* smem_a = smem;
   uint8_t* smem_b = smem + F8_STAGES * F8_A_BYTES;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + F8_STAGES * F8_STAGE_BYTES);
+  float* scratch = reinterpret_cast<float*>(smem + F8_STAGES * F8_STAGE_BYTES);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + F8_STAGES * F8_STAGE_BYTES + F8_SCR_BYTES);
   uint64_t* full_bar = bars;
   uint64_t* empty_bar = bars + F8_STAGES;
-  uint64_t* tmem_full = bars + 2 * F8_STAGES;
-  uint64_t* tmem_empty = tmem_full + 2;
-  uint32_t* tmem_base_smem = reinterpret_cast<uint32_t*>(tmem_empty + 2);
 
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int num_m = (p.M + F8_BM - 1) / F8_BM;
-  const int num_tiles = num_m * (p.N / F8_BN);
+  const int warp = threadIdx.x >> 5;
+  const int num_m = (p.M + F8_BM - 1) / F8_BM, num_n = p.N / F8_BN, num_tiles = num_m * num_n;
   const int num_k = (p.K + F8_BK - 1) / F8_BK;
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 256) {
     prefetch_tmap(&tmap_a);
     prefetch_tmap(&tmap_b);
-  }
-  if (warp == 1) {
-    if (lane == 0) {
-      for (int i = 0; i < F8_STAGES; ++i) {
-        mbar_init(&full_bar[i], 1);
-        mbar_init(&empty_bar[i], 1);
-      }
-      for (int i = 0; i < 2; ++i) {
-        mbar_init(&tmem_full[i], 1);
-        mbar_init(&tmem_empty[i], 4);
-      }
-      fence_barrier_init();
+    for (int i = 0; i < F8_STAGES; ++i) {
+      mbar_init(&full_bar[i], 1);
+      mbar_init(&empty_bar[i], 2);
     }
-    __syncwarp();
-    tmem_alloc<512>(tmem_base_smem);
+    fence_barrier_init();
   }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_base_smem;
 
-  if (warp == 0) {
-    if (elect_one()) {
+  if (warp >= 8) {
+    producer_regs();
+    if (warp == 8 && elect_one()) {
       int stage = 0;
       uint32_t phase = 0;
       for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
@@ -102,85 +77,22 @@ gemm_fp8_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constan
         }
       }
     }
-  } else if (warp == 1) {
-    if (elect_one()) {
-      // kind::f8f6f4 instruction descriptor: D f32, A / B e4m3 (format 0), both K-major
-      constexpr uint32_t idesc = make_idesc_ab(F8_BM, F8_BN, 0u, 0u, 0, 0);
-      const uint64_t desc_hi = make_smem_desc(0, 16, 1024) & 0xFFFFFFFF00000000ull;
-      const uint32_t desc_lo_c = static_cast<uint32_t>(make_smem_desc(0, 16, 1024));
-      const uint32_t a0 = smem_u32(smem_a), b0 = smem_u32(smem_b);
-      int stage = 0, acc = 0;
-      uint32_t phase = 0, acc_phase = 0;
-      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-        mbar_wait(&tmem_empty[acc], acc_phase ^ 1);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + acc * F8_BN;
-        for (int kb = 0; kb < num_k; ++kb) {
-          mbar_wait(&full_bar[stage], phase);
-          tc_fence_after();
-          const uint32_t a_lo = desc_lo_c | (((a0 + stage * F8_A_BYTES) & 0x3FFFF) >> 4);
-          const uint32_t b_lo = desc_lo_c | (((b0 + stage * F8_B_BYTES) & 0x3FFFF) >> 4);
-#pragma unroll
-          for (int k = 0; k < F8_BK / F8_UK; ++k)      // 32 bytes per k-step -> start address + 2 (x16 B)
-            umma_ss_f8(d_tmem, desc_hi | (a_lo + k * 2), desc_hi | (b_lo + k * 2), idesc, (kb | k) != 0 ? 1u : 0u);
-          umma_commit(&empty_bar[stage]);
-          if (kb == num_k - 1) umma_commit(&tmem_full[acc]);
-          if (++stage == F8_STAGES) {
-            stage = 0;
-            phase ^= 1;
-          }
-        }
-        if (++acc == 2) {
-          acc = 0;
-          acc_phase ^= 1;
-        }
-      }
-    }
-  } else {
-    const int quarter = warp & 3;
-    const float s = __ldg(scale_a) * scale_w;       // dequantisation: per-tensor activation x weight scale
-    int acc = 0;
-    uint32_t acc_phase = 0;
-    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-      const int m_blk = tile % num_m, n_blk = tile / num_m;
-      const int row = m_blk * F8_BM + quarter * 32 + lane;
-      const bool row_ok = row < p.M;
-      mbar_wait(&tmem_full[acc], acc_phase);
-      tc_fence_after();
-      const uint32_t t_row = tmem_base + (static_cast<uint32_t>(quarter * 32) << 16) + acc * F8_BN;
-      const uint16_t* gate_row = nullptr;
-      if constexpr (kEpi == EPI_BIAS_GATE_RES) {
-        const int g = row_ok ? (row + p.row_offset) / p.rows_per_gate : 0;
-        gate_row = reinterpret_cast<const uint16_t*>(p.gate) + static_cast<size_t>(g) * p.gate_stride;
-      }
-#pragma unroll 1
-      for (int c = 0; c < F8_BN / 32; ++c) {
-        uint32_t r[32];
-        tmem_ld_x32(t_row + c * 32, r);
-        tmem_ld_wait();
-        if (c == F8_BN / 32 - 1) {
-          tc_fence_before();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(&tmem_empty[acc]);
-        }
-        if (row_ok) {
-          float v[32];
-#pragma unroll
-          for (int j = 0; j < 32; ++j) v[j] = __uint_as_float(r[j]) * s;
-          gemm_epilogue_row32<true, kEpi>(v, row, n_blk * F8_BN + c * 32, p, gate_row);
-        }
-      }
-      if (++acc == 2) {
-        acc = 0;
-        acc_phase ^= 1;
-      }
-    }
+    return;
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc<512>(tmem_base);
+  consumer_regs();
+  const int wg = warp >> 2;
+  const uint32_t a_base = smem_u32(smem_a) + wg * 64 * F8_BK, b_base = smem_u32(smem_b);
+  float* scr = scratch + warp * kEpiScrFloats;
+  const float s = __ldg(scale_a) * scale_w;       // dequantisation: per-tensor activation x weight scale
+  int stage = 0;
+  uint32_t phase = 0;
+  for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+    const int m_blk = tile % num_m, n_blk = tile / num_m;
+    float acc[F8_BN / 2];
+    gemm_mainloop<F8_BN, 2>(acc, a_base, b_base, F8_A_BYTES, F8_B_BYTES, F8_STAGES, full_bar, empty_bar, stage, phase,
+                            0, num_k);
+    gemm_frag_epilogue<F8_BN, true, kEpi>(acc, scr, m_blk * F8_BM + wg * 64 + (warp & 3) * 16, n_blk * F8_BN, F8_BN,
+                                          s, p);
   }
 }
 
@@ -302,7 +214,7 @@ int gemm_fp8_tn(int epi, const void* a, int lda, const void* w, int ldw, const G
                 float scale_w, cudaStream_t stream) {
   if (p.M <= 0 || p.N <= 0 || p.K <= 0 || p.N % F8_BN != 0 || p.K % 16 != 0 || lda % 16 != 0 || ldw % 16 != 0 ||
       p.ldc % 8 != 0) {
-    set_last_error("gemm_fp8: unsupported shape M=%d N=%d K=%d (need N %% 256 == 0, K / ld %% 16 == 0)", p.M, p.N, p.K);
+    set_last_error("gemm_fp8: unsupported shape M=%d N=%d K=%d (need N %% 128 == 0, K / ld %% 16 == 0)", p.M, p.N, p.K);
     return KR_ERR_UNSUPPORTED_SHAPE;
   }
   if ((epi == EPI_BIAS_GATE_RES || epi == EPI_BIAS_RES || epi == EPI_MUL) && p.residual == nullptr) {

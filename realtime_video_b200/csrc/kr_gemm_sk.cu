@@ -1,21 +1,21 @@
-// kr_gemm_sk.cu — stream-K variant of the persistent tcgen05 GEMM (kr_gemm.cu) for shapes whose output-tile
-// count does not fill the 148 SMs evenly.
+// kr_gemm_sk.cu — stream-K variant of the persistent wgmma GEMM (kr_gemm.cu) for shapes whose output-tile
+// count does not fill the SMs evenly.
 //
 //   C[M,N] = epilogue( A[M,K] @ W[N,K]^T + bias[N] )        same operands / epilogues as kr_gemm.cu
 //
 // Why: the data-parallel kernels give every CTA whole 128x256 output tiles.  A sequence-parallel rank of the
-// multi-GPU mode owns M = 4680/N token rows (585 at 8 GPUs): to_qkv is then 5 x 60 = 300 tiles = 2.03 waves of
-// 148 CTAs (a third wave for 4 tiles), the o / cross-attention / ffn.2 projections are 100 tiles (0.68 of a wave).
+// multi-GPU mode owns M = 4680/N token rows (585 at 8 GPUs): to_qkv is then 5 x 60 = 300 tiles = 2.27 waves of
+// 132 CTAs (a third wave for 36 tiles), the o / cross-attention / ffn.2 projections are 100 tiles (0.76 of a wave).
 // Here the unit of work is one (tile, 64-wide k-block) MMA iteration: the num_tiles * num_k iterations are cut
-// into 148 equal contiguous ranges, so every SM runs the same number of tcgen05.mma k-blocks (+-1) whatever the
+// into one equal contiguous range per SM, so every SM runs the same number of k-blocks (+-1) whatever the
 // tile count.  A range that starts or ends inside a tile yields a PARTIAL accumulator:
 //   * every contributor of a split tile writes its fp32 partial (raw accumulator, 128 x 256) to its own slot of a
 //     workspace in HBM/L2 (slot 2*cta + {0 first segment, 1 last segment}), fences, and bumps the tile's counter;
 //   * the contributor that arrives last (counter == contributors - 1) re-reads all partials of the tile with
 //     L1-bypassing loads, sums them in ascending CTA order (deterministic) and runs the fused epilogue.
-// Tiles that one CTA covers completely take the data-parallel path (TMEM -> registers -> epilogue) untouched.
-// Roles / pipelines are those of kr_gemm.cu: warp 0 TMA producer (128x64 A + 256x64 W per stage, SWIZZLE_128B,
-// 4-stage ring), warp 1 one elected tcgen05.mma issuer, warps 2-5 epilogue, TMEM accumulators double-buffered.
+// Tiles that one CTA covers completely take the data-parallel path (registers -> epilogue) untouched.
+// Roles / pipelines are those of kr_gemm.cu: two consumer warpgroups (wgmma on 64 rows each, then the epilogue),
+// warp 8 the TMA producer (warps 8..11 hand their registers to the consumers) (128x64 A + 256x64 W per stage, SWIZZLE_128B, 4-stage ring).
 #include "kr_common.cuh"
 #include "kr_gemm_epi.cuh"
 #include "kr_ops.h"
@@ -23,13 +23,13 @@
 namespace kr {
 
 namespace {
-constexpr int SK_BM = 128, SK_BN = 256, SK_BK = 64, SK_UK = 16;
-constexpr int SK_THREADS = 192;
+constexpr int SK_BM = 128, SK_BN = 256, SK_BK = 64;
+constexpr int SK_THREADS = 384;
 constexpr int SK_STAGES = 4;
 constexpr int SK_A_BYTES = SK_BM * SK_BK * 2, SK_B_BYTES = SK_BN * SK_BK * 2;
 constexpr int SK_STAGE_BYTES = SK_A_BYTES + SK_B_BYTES;
-constexpr int SK_SMEM = SK_STAGES * SK_STAGE_BYTES + 1024 + 256;
-constexpr int SK_TMEM_COLS = 2 * SK_BN;
+constexpr int SK_SCR_BYTES = 8 * kEpiScrFloats * 4;
+constexpr int SK_SMEM = SK_STAGES * SK_STAGE_BYTES + SK_SCR_BYTES + 1024 + 256;
 constexpr size_t SK_SLOT_FLOATS = static_cast<size_t>(SK_BM) * SK_BN;
 constexpr size_t SK_COUNTER_BYTES = 64 * 1024;      // 16384 tile counters in front of the partial slots
 
@@ -59,45 +59,31 @@ gemm_sk_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
                                              ~static_cast<uintptr_t>(1023));
   uint8_t* smem_a = smem;
   uint8_t* smem_b = smem + SK_STAGES * SK_A_BYTES;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + SK_STAGES * SK_STAGE_BYTES);
+  float* scratch = reinterpret_cast<float*>(smem + SK_STAGES * SK_STAGE_BYTES);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + SK_STAGES * SK_STAGE_BYTES + SK_SCR_BYTES);
   uint64_t* full_bar = bars;
   uint64_t* empty_bar = bars + SK_STAGES;
-  uint64_t* tmem_full = bars + 2 * SK_STAGES;
-  uint64_t* tmem_empty = tmem_full + 2;
-  uint32_t* tmem_base_smem = reinterpret_cast<uint32_t*>(tmem_empty + 2);
-  volatile int* last_flag = reinterpret_cast<volatile int*>(tmem_base_smem + 1);
+  volatile int* last_flag = reinterpret_cast<volatile int*>(empty_bar + SK_STAGES);
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
   const long long it_begin = sk_begin(s, blockIdx.x), it_end = sk_begin(s, blockIdx.x + 1);
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 256) {
     prefetch_tmap(&tmap_a);
     prefetch_tmap(&tmap_b);
-  }
-  if (warp == 1) {
-    if (lane == 0) {
-      for (int i = 0; i < SK_STAGES; ++i) {
-        mbar_init(&full_bar[i], 1);
-        mbar_init(&empty_bar[i], 1);
-      }
-      for (int i = 0; i < 2; ++i) {
-        mbar_init(&tmem_full[i], 1);
-        mbar_init(&tmem_empty[i], 4);
-      }
-      fence_barrier_init();
+    for (int i = 0; i < SK_STAGES; ++i) {
+      mbar_init(&full_bar[i], 1);
+      mbar_init(&empty_bar[i], 2);
     }
-    __syncwarp();
-    tmem_alloc<SK_TMEM_COLS>(tmem_base_smem);
+    fence_barrier_init();
   }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_base_smem;
 
-  if (warp == 0) {
-    // ===================== TMA producer =====================
-    if (elect_one()) {
+  if (warp >= 8) {
+    // ===================== TMA producer (warp 8; warps 9..11 only give their registers back) =====================
+    producer_regs();
+    if (warp == 8 && elect_one()) {
       int stage = 0;
       uint32_t phase = 0;
       for (long long it = it_begin; it < it_end;) {
@@ -119,53 +105,15 @@ gemm_sk_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
         it += k1 - k0;
       }
     }
-  } else if (warp == 1) {
-    // ===================== MMA issuer =====================
-    if (elect_one()) {
-      constexpr uint32_t idesc = make_idesc<kBf16>(SK_BM, SK_BN, 0, 0);
-      const uint64_t desc_hi = make_smem_desc(0, 16, 1024) & 0xFFFFFFFF00000000ull;
-      const uint32_t desc_lo_c = static_cast<uint32_t>(make_smem_desc(0, 16, 1024));
-      const uint32_t a0 = smem_u32(smem_a), b0 = smem_u32(smem_b);
-      int stage = 0, acc = 0;
-      uint32_t phase = 0, acc_phase = 0;
-      for (long long it = it_begin; it < it_end;) {
-        const int tile = static_cast<int>(it / s.num_k);
-        const int k0 = static_cast<int>(it - static_cast<long long>(tile) * s.num_k);
-        const long long left = it_end - it;
-        const int k1 = (s.num_k - k0) < left ? s.num_k : k0 + static_cast<int>(left);
-        mbar_wait(&tmem_empty[acc], acc_phase ^ 1);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + acc * SK_BN;
-        for (int kb = k0; kb < k1; ++kb) {
-          mbar_wait(&full_bar[stage], phase);
-          tc_fence_after();
-          const uint32_t a_lo = desc_lo_c | (((a0 + stage * SK_A_BYTES) & 0x3FFFF) >> 4);
-          const uint32_t b_lo = desc_lo_c | (((b0 + stage * SK_B_BYTES) & 0x3FFFF) >> 4);
-#pragma unroll
-          for (int k = 0; k < SK_BK / SK_UK; ++k) {
-            umma_ss(d_tmem, desc_hi | (a_lo + k * 2), desc_hi | (b_lo + k * 2), idesc,
-                    (kb != k0 || k != 0) ? 1u : 0u);
-          }
-          umma_commit(&empty_bar[stage]);
-          if (kb == k1 - 1) umma_commit(&tmem_full[acc]);
-          if (++stage == SK_STAGES) {
-            stage = 0;
-            phase ^= 1;
-          }
-        }
-        if (++acc == 2) {
-          acc = 0;
-          acc_phase ^= 1;
-        }
-        it += k1 - k0;
-      }
-    }
   } else {
-    // ===================== epilogue warps =====================
-    const int quarter = warp & 3;
-    const int etid = threadIdx.x - 64;          // 0..127 among the epilogue threads
-    int acc = 0, seg = 0;
-    uint32_t acc_phase = 0;
+    // ===================== consumer warpgroups =====================
+    consumer_regs();
+    const int wg = warp >> 2;
+    const int etid = threadIdx.x;                // 0..255 among the consumer threads
+    const uint32_t a_base = smem_u32(smem_a) + wg * 64 * 128, b_base = smem_u32(smem_b);
+    float* scr = scratch + warp * kEpiScrFloats;
+    int stage = 0, seg = 0;
+    uint32_t phase = 0;
     for (long long it = it_begin; it < it_end; ++seg) {
       const int tile = static_cast<int>(it / s.num_k);
       const int k0 = static_cast<int>(it - static_cast<long long>(tile) * s.num_k);
@@ -173,106 +121,73 @@ gemm_sk_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
       const int k1 = (s.num_k - k0) < left ? s.num_k : k0 + static_cast<int>(left);
       it += k1 - k0;
       const int m_blk = tile % s.num_m, n_blk = tile / s.num_m;
-      const int lrow = quarter * 32 + lane;
-      const int row = m_blk * SK_BM + lrow;
-      const bool row_ok = row < p.M;
-      mbar_wait(&tmem_full[acc], acc_phase);
-      tc_fence_after();
-      const uint32_t t_row = tmem_base + (static_cast<uint32_t>(quarter * 32) << 16) + acc * SK_BN;
-      const uint16_t* gate_row = nullptr;
-      if constexpr (kEpi == EPI_BIAS_GATE_RES) {
-        const int g = row_ok ? (row + p.row_offset) / p.rows_per_gate : 0;
-        gate_row = reinterpret_cast<const uint16_t*>(p.gate) + static_cast<size_t>(g) * p.gate_stride;
+      float acc[SK_BN / 2];
+      gemm_mainloop<SK_BN, kBf16 ? 0 : 1>(acc, a_base, b_base, SK_A_BYTES, SK_B_BYTES, SK_STAGES, full_bar,
+                                          empty_bar, stage, phase, k0, k1);
+      if (k0 == 0 && k1 == s.num_k) {
+        gemm_frag_epilogue<SK_BN, kBf16, kEpi>(acc, scr, m_blk * SK_BM + wg * 64 + (warp & 3) * 16, n_blk * SK_BN,
+                                               SK_BN, 1.0f, p);
+        continue;
       }
-      const bool whole = (k0 == 0 && k1 == s.num_k);
-      if (whole) {
-#pragma unroll 1
-        for (int c = 0; c < SK_BN / 32; ++c) {
-          uint32_t r[32];
-          tmem_ld_x32(t_row + c * 32, r);
-          tmem_ld_wait();
-          if (c == SK_BN / 32 - 1) {
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&tmem_empty[acc]);
+      // ---- partial accumulator -> my workspace slot ([128][256] fp32, fragment by fragment) ----
+      float* mine = s.slots + static_cast<size_t>(2 * blockIdx.x + (seg == 0 ? 0 : 1)) * SK_SLOT_FLOATS;
+      {
+        const int r = wg * 64 + (warp & 3) * 16 + (lane >> 2);
+#pragma unroll
+        for (int j = 0; j < SK_BN / 8; ++j) {
+          const int col = j * 8 + 2 * (lane & 3);
+          __stcg(reinterpret_cast<float2*>(mine + static_cast<size_t>(r) * SK_BN + col),
+                 make_float2(acc[4 * j], acc[4 * j + 1]));
+          __stcg(reinterpret_cast<float2*>(mine + static_cast<size_t>(r + 8) * SK_BN + col),
+                 make_float2(acc[4 * j + 2], acc[4 * j + 3]));
+        }
+      }
+      __threadfence();
+      // contributors of this tile: the CTAs whose ranges intersect [tile*num_k, (tile+1)*num_k)
+      const long long t0 = static_cast<long long>(tile) * s.num_k;
+      const int c_first = sk_cta_of(s, t0), c_last = sk_cta_of(s, t0 + s.num_k - 1);
+      named_bar_sync(1, 256);
+      if (etid == 0) {
+        const int old = atomicAdd(s.counters + tile, 1);
+        const int last = (old == c_last - c_first) ? 1 : 0;
+        if (last) s.counters[tile] = 0;            // ready for the next launch
+        *last_flag = last;
+      }
+      named_bar_sync(1, 256);
+      const bool is_last = *last_flag != 0;
+      named_bar_sync(1, 256);   // flag consumed before the next segment rewrites it
+      if (is_last) {
+        __threadfence();
+        // thread = (row, half of the columns); partials summed in ascending CTA order
+        const int lrow = etid >> 1, half = etid & 1;
+        const int row = m_blk * SK_BM + lrow;
+        if (row < p.M) {
+          const uint16_t* gate_row = nullptr;
+          if constexpr (kEpi == EPI_BIAS_GATE_RES) {
+            const int g = (row + p.row_offset) / p.rows_per_gate;
+            gate_row = reinterpret_cast<const uint16_t*>(p.gate) + static_cast<size_t>(g) * p.gate_stride;
           }
-          if (row_ok) {
+#pragma unroll 1
+          for (int c = half * 4; c < half * 4 + 4; ++c) {
             float v[32];
 #pragma unroll
-            for (int j = 0; j < 32; ++j) v[j] = __uint_as_float(r[j]);
-            gemm_epilogue_row32<kBf16, kEpi>(v, row, n_blk * SK_BN + c * 32, p, gate_row);
-          }
-        }
-      } else {
-        // ---- partial accumulator -> my workspace slot ----
-        float* mine = s.slots + (static_cast<size_t>(2 * blockIdx.x + (seg == 0 ? 0 : 1)) * SK_SLOT_FLOATS) +
-                      static_cast<size_t>(lrow) * SK_BN;
-#pragma unroll 1
-        for (int c = 0; c < SK_BN / 32; ++c) {
-          uint32_t r[32];
-          tmem_ld_x32(t_row + c * 32, r);
-          tmem_ld_wait();
-          if (c == SK_BN / 32 - 1) {
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&tmem_empty[acc]);
-          }
-          float4* dst = reinterpret_cast<float4*>(mine + c * 32);
+            for (int j = 0; j < 32; ++j) v[j] = 0.f;
+            for (int cc = c_first; cc <= c_last; ++cc) {
+              // tile is cc's first segment iff cc's range starts inside (or at the start of) this tile
+              const int sl = 2 * cc + (sk_begin(s, cc) >= t0 ? 0 : 1);
+              const float4* src = reinterpret_cast<const float4*>(
+                  s.slots + static_cast<size_t>(sl) * SK_SLOT_FLOATS + static_cast<size_t>(lrow) * SK_BN + c * 32);
 #pragma unroll
-          for (int j = 0; j < 8; ++j)
-            __stcg(dst + j, make_float4(__uint_as_float(r[4 * j]), __uint_as_float(r[4 * j + 1]),
-                                        __uint_as_float(r[4 * j + 2]), __uint_as_float(r[4 * j + 3])));
-        }
-        __threadfence();
-        // contributors of this tile: the CTAs whose ranges intersect [tile*num_k, (tile+1)*num_k)
-        const long long t0 = static_cast<long long>(tile) * s.num_k;
-        const int c_first = sk_cta_of(s, t0), c_last = sk_cta_of(s, t0 + s.num_k - 1);
-        asm volatile("bar.sync 1, 128;" ::: "memory");
-        if (etid == 0) {
-          const int old = atomicAdd(s.counters + tile, 1);
-          const int last = (old == c_last - c_first) ? 1 : 0;
-          if (last) s.counters[tile] = 0;            // ready for the next launch
-          *last_flag = last;
-        }
-        asm volatile("bar.sync 1, 128;" ::: "memory");
-        const bool is_last = *last_flag != 0;
-        asm volatile("bar.sync 1, 128;" ::: "memory");   // flag consumed before the next segment rewrites it
-        if (is_last) {
-          __threadfence();
-          if (row_ok) {
-#pragma unroll 1
-            for (int c = 0; c < SK_BN / 32; ++c) {
-              float v[32];
-#pragma unroll
-              for (int j = 0; j < 32; ++j) v[j] = 0.f;
-              for (int cc = c_first; cc <= c_last; ++cc) {
-                // tile is cc's first segment iff cc's range starts inside (or at the start of) this tile
-                const int sl = 2 * cc + (sk_begin(s, cc) >= t0 ? 0 : 1);
-                const float4* src = reinterpret_cast<const float4*>(
-                    s.slots + static_cast<size_t>(sl) * SK_SLOT_FLOATS + static_cast<size_t>(lrow) * SK_BN + c * 32);
-#pragma unroll
-                for (int j = 0; j < 8; ++j) {
-                  const float4 f = __ldcg(src + j);
-                  v[4 * j] += f.x; v[4 * j + 1] += f.y; v[4 * j + 2] += f.z; v[4 * j + 3] += f.w;
-                }
+              for (int j = 0; j < 8; ++j) {
+                const float4 f = __ldcg(src + j);
+                v[4 * j] += f.x; v[4 * j + 1] += f.y; v[4 * j + 2] += f.z; v[4 * j + 3] += f.w;
               }
-              gemm_epilogue_row32<kBf16, kEpi>(v, row, n_blk * SK_BN + c * 32, p, gate_row);
             }
+            gemm_epilogue_row<kBf16, kEpi, 32>(v, row, n_blk * SK_BN + c * 32, p, gate_row);
           }
         }
-      }
-      if (++acc == 2) {
-        acc = 0;
-        acc_phase ^= 1;
       }
     }
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc<SK_TMEM_COLS>(tmem_base);
   }
 }
 

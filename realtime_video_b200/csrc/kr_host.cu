@@ -23,10 +23,10 @@ int sm_count() {
   static int cached = 0;
   if (cached == 0) {
     int dev = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess) return 148;
+    if (cudaGetDevice(&dev) != cudaSuccess) return 132;
     int n = 0;
     if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0)
-      return 148;
+      return 132;
     cached = n;
   }
   return cached;

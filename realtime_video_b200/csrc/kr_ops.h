@@ -42,16 +42,15 @@ int gemm_sk_tn(int dtype, int epi, const void* a, int lda, const void* w, int ld
                void* workspace, size_t workspace_bytes, cudaStream_t stream);
 size_t gemm_sk_workspace_bytes();
 bool gemm_sk_preferred(int epi, int M, int N, int K);
-// FP8 (e4m3) path, kr_gemm_fp8.cu: dynamic per-tensor activation quantisation + kind::f8f6f4 GEMM.
+// FP8 (e4m3) path, kr_gemm_fp8.cu: dynamic per-tensor activation quantisation + e4m3 wgmma GEMM.
 // state: 2 floats of device memory [amax, dequant scale = amax / 448]; the GEMM reads state[1] as scale_a.
 int fp8_quantize(const void* x, long ld, int rows, int cols, void* q, long ldq, float* state, cudaStream_t stream);
 int gemm_fp8_tn(int epi, const void* a, int lda, const void* w, int ldw, const GemmParams& p, const float* scale_a,
                 float scale_w, cudaStream_t stream);
-// CTA-pair (cta_group::2, 256x256 tiles) variant, kr_gemm2.cu
+// 2-CTA cluster variant (W multicast to both CTAs, 128x256 tile per CTA), kr_gemm2.cu; N % 256 == 0
 int gemm2_tn(int dtype, int epi, const void* a, int lda, const void* w, int ldw, const GemmParams& p,
              cudaStream_t stream);
-bool gemm_uses_pair(int epi, int M, int N, int K);
-int gemm_plan(int epi, int M, int N, int K, bool have_workspace = false);   // 0 single-CTA kernel, 1 CTA-pair kernel, 2 stream-K, 3 single-CTA kernel with a wave-fitted runtime tile width
+int gemm_plan(int epi, int M, int N, int K, bool have_workspace = false);   // 0 fixed-width kernel, 1 2-CTA cluster kernel, 2 stream-K, 3 runtime-width kernel
 int gemm_flex_bn(int epi, int M, int N, int K);
 
 struct AttnParams {

@@ -1,23 +1,22 @@
-// kr_t5attn.cu — tcgen05/TMEM attention for the UMT5 text encoder: head_dim 64, additive relative-position
+// kr_t5attn.cu — wgmma attention for the UMT5 text encoder: head_dim 64, additive relative-position
 // bias, key-padding mask, no 1/sqrt(d) scaling.
 //
 //   O[q, h, :] = softmax_k( bf16(bf16(Q[q,h,:] . K[k,h,:]) + bias[h, k - q]) ) V[k, h, :]
 //
 // Replaces, on the reference path, T5Attention.forward (wan/modules/t5.py:86-120): the two einsums, the
 // [B, heads, L, L] bias tensor (pos_bias of T5RelativeEmbedding :221-264 + masked_fill with finfo.min) and the
-// fp32 softmax — round-1 ran it as 64 heads x (GEMM, eager add, softmax kernel, GEMM) with the L x L scores in HBM.
+// fp32 softmax.
 // The position bias only depends on (head, k - q): the host gathers it once per layer into `bias_delta`
 // [heads, 2L-1] (entry d = embedding[bucket(d - (L-1))][head]) and the kernel keeps one head's row in shared memory.
 // Rounding points follow the reference's bf16 execution: the einsum output is rounded to bf16, the bias add is a
 // bf16 add, the softmax runs in fp32 and P is rounded to bf16 before P.V (here un-normalised, flash style; the
 // 1/rowsum is applied to the fp32 output).
 //
-// CTA = 128 query rows of one head; key tiles of 256 (online softmax across tiles, L = 512 -> 2 tiles):
-//   warp 0 (one elected thread): TMA loads (Q 128x64, K/V 256x64 per tile, 2 stages) and every tcgen05.mma
-//   warps 4..7: softmax, one thread per query row, S read from TMEM in 32-column chunks (two passes: max, then exp)
-// TMEM: S fp32 [128 x 256] at columns 0..255, P (bf16, 2 per column) aliases columns 0..127, O fp32 at 256..319.
+// CTA = 128 query rows of one head; key tiles of 128 (online softmax across tiles):
+//   warps 0..7: two consumer warpgroups (64 query rows each): S = Q.K^T and O += P.V with wgmma, softmax in registers
+//   warps 8..11: TMA warpgroup (Q 128x64 once, K/V 128x64 tiles through a 4-stage ring K0 V0 K1 V1 ...)
 // The op is 4.3 GFLOP per encoder layer (0.1 % of the encoder): the design goal is "one launch, nothing in HBM but
-// q/k/v/o", not pipelining — S(j+1) is issued after P.V(j) retires.
+// q/k/v/o".
 #include "kr_common.cuh"
 #include "kr_ops.h"
 
@@ -26,10 +25,10 @@
 namespace kr {
 
 namespace {
-constexpr int T5_D = 64, T5_TQ = 128, T5_TK = 256, T5_THREADS = 256;
+constexpr int T5_D = 64, T5_TQ = 128, T5_TK = 128, T5_THREADS = 384, T5_STAGES = 4;
 constexpr int T5_Q_BYTES = T5_TQ * T5_D * 2, T5_KV_BYTES = T5_TK * T5_D * 2;
 constexpr int T5_MAX_L = 1024;
-constexpr int T5_SMEM = T5_Q_BYTES + 4 * T5_KV_BYTES + (2 * T5_MAX_L) * 2 + T5_MAX_L + 1024 + 256;
+constexpr int T5_SMEM = T5_Q_BYTES + T5_STAGES * T5_KV_BYTES + (2 * T5_MAX_L) * 2 + T5_MAX_L + 1024 + 256;
 }  // namespace
 
 __global__ void __launch_bounds__(T5_THREADS, 1)
@@ -39,18 +38,13 @@ t5_attn_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
                                              ~static_cast<uintptr_t>(1023));
   uint8_t* smem_q = smem;
-  uint8_t* smem_k = smem + T5_Q_BYTES;                   // 2 stages
-  uint8_t* smem_v = smem_k + 2 * T5_KV_BYTES;            // 2 stages
-  uint16_t* bias_s = reinterpret_cast<uint16_t*>(smem_v + 2 * T5_KV_BYTES);      // [2L-1]
+  uint8_t* smem_kv = smem + T5_Q_BYTES;                                          // T5_STAGES tiles
+  uint16_t* bias_s = reinterpret_cast<uint16_t*>(smem_kv + T5_STAGES * T5_KV_BYTES);   // [2L-1]
   uint8_t* mask_s = reinterpret_cast<uint8_t*>(bias_s + 2 * T5_MAX_L);           // [L]
   uint64_t* bars = reinterpret_cast<uint64_t*>(mask_s + T5_MAX_L);
-  uint64_t* q_full = bars;          // [1]
-  uint64_t* k_full = bars + 1;      // [2]
-  uint64_t* v_full = bars + 3;      // [2]
-  uint64_t* s_full = bars + 5;      // [1]
-  uint64_t* p_ready = bars + 6;     // [1] 4 arrivals (one per softmax warp)
-  uint64_t* o_done = bars + 7;      // [1]
-  uint32_t* tmem_base_smem = reinterpret_cast<uint32_t*>(bars + 8);
+  uint64_t* q_full = bars;                     // [1]
+  uint64_t* kv_full = bars + 1;                // [T5_STAGES]
+  uint64_t* kv_empty = kv_full + T5_STAGES;    // [T5_STAGES]
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int nqb = (p.L + T5_TQ - 1) / T5_TQ;
@@ -58,25 +52,16 @@ t5_attn_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant
   const int n_tiles = (p.L + T5_TK - 1) / T5_TK;
   const int col = head * T5_D;
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 256) {
     prefetch_tmap(&tmap_q);
     prefetch_tmap(&tmap_k);
     prefetch_tmap(&tmap_v);
-  }
-  if (warp == 1) {
-    if (lane == 0) {
-      mbar_init(q_full, 1);
-      for (int i = 0; i < 2; ++i) {
-        mbar_init(&k_full[i], 1);
-        mbar_init(&v_full[i], 1);
-      }
-      mbar_init(s_full, 1);
-      mbar_init(p_ready, 4);
-      mbar_init(o_done, 1);
-      fence_barrier_init();
+    mbar_init(q_full, 1);
+    for (int i = 0; i < T5_STAGES; ++i) {
+      mbar_init(&kv_full[i], 1);
+      mbar_init(&kv_empty[i], 2);
     }
-    __syncwarp();
-    tmem_alloc<512>(tmem_base_smem);
+    fence_barrier_init();
   }
   // this head's bias row and the key mask -> shared memory (all threads)
   {
@@ -85,156 +70,129 @@ t5_attn_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant
     for (int i = threadIdx.x; i < p.L; i += T5_THREADS)
       mask_s[i] = p.key_mask != nullptr ? reinterpret_cast<const uint8_t*>(p.key_mask)[i] : 1;
   }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_base_smem;
-  const uint32_t tS = tmem_base, tO = tmem_base + 256;
 
-  if (warp == 0) {
-    if (elect_one()) {
-      auto load_kv = [&](int j) {
-        const int s = j & 1;
-        mbar_expect_tx(&k_full[s], T5_KV_BYTES);
-        tma_load_2d(smem_k + s * T5_KV_BYTES, &tmap_k, &k_full[s], col, j * T5_TK);
-        mbar_expect_tx(&v_full[s], T5_KV_BYTES);
-        tma_load_2d(smem_v + s * T5_KV_BYTES, &tmap_v, &v_full[s], col, j * T5_TK);
-      };
+  auto st = [](int item) { return item % T5_STAGES; };
+  auto ph = [](int item) { return static_cast<uint32_t>((item / T5_STAGES) & 1); };
+
+  if (warp >= 8) {
+    producer_regs();
+    if (warp == 8 && elect_one()) {
       mbar_expect_tx(q_full, T5_Q_BYTES);
       tma_load_2d(smem_q, &tmap_q, q_full, col, q0);
-      load_kv(0);
-      if (n_tiles > 1) load_kv(1);
-      constexpr uint32_t idesc_qk = make_idesc<true>(T5_TQ, T5_TK, 0, 0);
-      constexpr uint32_t idesc_pv = make_idesc_ab(T5_TQ, T5_D, 1u, 1u, 0, 1);
-      const uint32_t qa = smem_u32(smem_q);
-      mbar_wait(q_full, 0);
-      for (int j = 0; j < n_tiles; ++j) {
-        const int s = j & 1;
-        const uint32_t par = static_cast<uint32_t>((j >> 1) & 1);
-        const uint32_t ka = smem_u32(smem_k + s * T5_KV_BYTES), va = smem_u32(smem_v + s * T5_KV_BYTES);
-        mbar_wait(&k_full[s], par);
-        tc_fence_after();
-#pragma unroll
-        for (int k = 0; k < T5_D / 16; ++k)
-          umma_ss(tS, make_smem_desc(qa + k * 32, 16, 1024), make_smem_desc(ka + k * 32, 16, 1024), idesc_qk,
-                  k != 0 ? 1u : 0u);
-        umma_commit(s_full);
-        mbar_wait(p_ready, static_cast<uint32_t>(j & 1));
-        mbar_wait(&v_full[s], par);
-        tc_fence_after();
-#pragma unroll
-        for (int k = 0; k < T5_TK / 16; ++k)
-          umma_ts(tO, tS + k * 8, make_smem_desc(va + k * 2048, 1024, 1024), idesc_pv, (j == 0 && k == 0) ? 0u : 1u);
-        umma_commit(o_done);
-        mbar_wait(o_done, static_cast<uint32_t>(j & 1));       // S / P buffer and this stage are free again
-        if (j + 2 < n_tiles) load_kv(j + 2);
+      for (int it = 0; it < 2 * n_tiles; ++it) {
+        mbar_wait(&kv_empty[st(it)], ph(it) ^ 1);
+        mbar_expect_tx(&kv_full[st(it)], T5_KV_BYTES);
+        tma_load_2d(smem_kv + st(it) * T5_KV_BYTES, (it & 1) ? &tmap_v : &tmap_k, &kv_full[st(it)], col,
+                    (it >> 1) * T5_TK);
       }
     }
-    __syncwarp();
-  } else if (warp >= 4) {
-    const int quarter = warp & 3;
-    const int q_row = q0 + quarter * 32 + lane;
-    const uint32_t lane_off = static_cast<uint32_t>(quarter * 32) << 16;
-    const uint32_t tSr = tS + lane_off, tOr = tO + lane_off;
-    const float kLog2e = 1.4426950408889634f;
-    const float kMin = -3.3895313892515355e38f;     // torch.finfo(torch.bfloat16).min
-    float m_run = -INFINITY, l_run = 0.f;
-    const int qq = q_row < p.L ? q_row : p.L - 1;
-
-    // one chunk of 32 scores of this row -> the reference's bf16(bf16(s) + bias), masked keys = finfo.min
-    auto scores = [&](const uint32_t (&r)[32], int k0, float (&x)[32]) {
-#pragma unroll
-      for (int c = 0; c < 32; ++c) {
-        const int k = k0 + c;
-        float v = -INFINITY;                                   // key rows past L (TMA zero fill)
-        if (k < p.L) {
-          const float b = __bfloat162float(__ushort_as_bfloat16(bias_s[k - qq + p.L - 1]));
-          v = mask_s[k] ? bf16_round(bf16_round(__uint_as_float(r[c])) + b) : kMin;
-        }
-        x[c] = v;
-      }
-    };
-
-    for (int j = 0; j < n_tiles; ++j) {
-      mbar_wait(s_full, static_cast<uint32_t>(j & 1));
-      tc_fence_after();
-      float mt = -INFINITY;
-#pragma unroll 1
-      for (int c = 0; c < T5_TK / 32; ++c) {
-        uint32_t r[32];
-        float x[32];
-        tmem_ld_x32(tSr + c * 32, r);
-        tmem_ld_wait();
-        scores(r, j * T5_TK + c * 32, x);
-#pragma unroll
-        for (int i = 0; i < 32; ++i) mt = fmaxf(mt, x[i]);
-      }
-      const float m_new = fmaxf(m_run, mt);
-      const float alpha = fast_exp2((m_run - m_new) * kLog2e);     // 0 on the first tile (m_run = -inf)
-      if (j > 0) {
-#pragma unroll 1
-        for (int c = 0; c < T5_D / 32; ++c) {
-          uint32_t o[32];
-          tmem_ld_x32(tOr + c * 32, o);
-          tmem_ld_wait();
-#pragma unroll
-          for (int i = 0; i < 32; ++i) o[i] = __float_as_uint(__uint_as_float(o[i]) * alpha);
-          tmem_st_x32(tOr + c * 32, o);
-        }
-      }
-      l_run *= alpha;
-      m_run = m_new;
-      const float nm = -m_new * kLog2e;
-#pragma unroll 1
-      for (int c = 0; c < T5_TK / 32; ++c) {
-        uint32_t r[32], pk[16];
-        float x[32];
-        tmem_ld_x32(tSr + c * 32, r);
-        tmem_ld_wait();
-        scores(r, j * T5_TK + c * 32, x);
-#pragma unroll
-        for (int i = 0; i < 16; ++i) {
-          const float a0 = fast_exp2(fmaf(x[2 * i], kLog2e, nm));
-          const float a1 = fast_exp2(fmaf(x[2 * i + 1], kLog2e, nm));
-          l_run += a0 + a1;
-          pk[i] = pack_bf16x2(a0, a1);
-        }
-        // P chunk c lives in columns [16c, 16c+16): S columns already consumed (chunks <= c, ascending order)
-        tmem_st_x16(tSr + c * 16, pk);
-      }
-      tmem_st_wait();
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(p_ready);
-    }
-    mbar_wait(o_done, static_cast<uint32_t>((n_tiles - 1) & 1));
-    tc_fence_after();
-    const float inv_l = 1.0f / l_run;
-    uint16_t* orow = reinterpret_cast<uint16_t*>(p.out) + static_cast<size_t>(qq) * p.ldo + col;
-#pragma unroll 1
-    for (int c = 0; c < T5_D / 32; ++c) {
-      uint32_t o[32];
-      tmem_ld_x32(tOr + c * 32, o);
-      tmem_ld_wait();
-      if (q_row < p.L) {
-#pragma unroll
-        for (int q = 0; q < 4; ++q) {
-          uint4 w;
-          w.x = pack_bf16x2(__uint_as_float(o[q * 8 + 0]) * inv_l, __uint_as_float(o[q * 8 + 1]) * inv_l);
-          w.y = pack_bf16x2(__uint_as_float(o[q * 8 + 2]) * inv_l, __uint_as_float(o[q * 8 + 3]) * inv_l);
-          w.z = pack_bf16x2(__uint_as_float(o[q * 8 + 4]) * inv_l, __uint_as_float(o[q * 8 + 5]) * inv_l);
-          w.w = pack_bf16x2(__uint_as_float(o[q * 8 + 6]) * inv_l, __uint_as_float(o[q * 8 + 7]) * inv_l);
-          reinterpret_cast<uint4*>(orow + c * 32)[q] = w;
-        }
-      }
-    }
+    return;
   }
 
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc<512>(tmem_base);
+  consumer_regs();
+  const int wg = warp >> 2;
+  const bool leader = (threadIdx.x & 127) == 0;
+  const uint32_t q_addr = smem_u32(smem_q) + wg * 64 * 128, kv_addr = smem_u32(smem_kv);
+  const float kLog2e = 1.4426950408889634f;
+  const float kMin = -3.3895313892515355e38f;     // torch.finfo(torch.bfloat16).min
+  int q_row[2], qq[2];
+#pragma unroll
+  for (int r = 0; r < 2; ++r) {
+    q_row[r] = q0 + wg * 64 + (warp & 3) * 16 + (lane >> 2) + 8 * r;
+    qq[r] = q_row[r] < p.L ? q_row[r] : p.L - 1;
+  }
+  float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};
+  float o[T5_D / 2];
+#pragma unroll
+  for (int i = 0; i < T5_D / 2; ++i) o[i] = 0.f;
+
+  mbar_wait(q_full, 0);
+  for (int j = 0; j < n_tiles; ++j) {
+    float s[T5_TK / 2];
+    mbar_wait(&kv_full[st(2 * j)], ph(2 * j));
+    {
+      const uint32_t b = kv_addr + st(2 * j) * T5_KV_BYTES;
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < T5_D / 16; ++k)
+        wgmma_ss<T5_TK, true, 0>(s, make_smem_desc(q_addr + k * 32, 16, 1024), make_smem_desc(b + k * 32, 16, 1024),
+                                 k != 0 ? 1 : 0);
+      wgmma_commit();
+      wgmma_wait<0>();
+      reg_fence(s);
+    }
+    if (leader) mbar_arrive(&kv_empty[st(2 * j)]);
+    // the reference's bf16(bf16(s) + bias), masked keys = finfo.min, key rows past L (TMA zero fill) = -inf
+    float nm[2];
+#pragma unroll
+    for (int r = 0; r < 2; ++r) {
+      float mt = -INFINITY;
+#pragma unroll
+      for (int nb = 0; nb < T5_TK / 8; ++nb)
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const int k = j * T5_TK + nb * 8 + 2 * (lane & 3) + e;
+          float v = -INFINITY;
+          if (k < p.L) {
+            const float b = __bfloat162float(__ushort_as_bfloat16(bias_s[k - qq[r] + p.L - 1]));
+            v = mask_s[k] ? bf16_round(bf16_round(s[4 * nb + 2 * r + e]) + b) : kMin;
+          }
+          s[4 * nb + 2 * r + e] = v;
+          mt = fmaxf(mt, v);
+        }
+      mt = fmaxf(mt, __shfl_xor_sync(0xffffffffu, mt, 1));
+      mt = fmaxf(mt, __shfl_xor_sync(0xffffffffu, mt, 2));
+      const float m_new = fmaxf(m_run[r], mt);
+      const float alpha = fast_exp2((m_run[r] - m_new) * kLog2e);     // 0 on the first tile (m_run = -inf)
+#pragma unroll
+      for (int nb = 0; nb < T5_D / 8; ++nb) {
+        o[4 * nb + 2 * r] *= alpha;
+        o[4 * nb + 2 * r + 1] *= alpha;
+      }
+      l_run[r] *= alpha;
+      m_run[r] = m_new;
+      nm[r] = -m_new * kLog2e;
+    }
+    uint32_t pa[T5_TK / 16][4];
+#pragma unroll
+    for (int kk = 0; kk < T5_TK / 16; ++kk)
+#pragma unroll
+      for (int h = 0; h < 2; ++h)
+#pragma unroll
+        for (int r = 0; r < 2; ++r) {
+          const int i = 8 * kk + 4 * h + 2 * r;
+          const float a0 = fast_exp2(fmaf(s[i], kLog2e, nm[r]));
+          const float a1 = fast_exp2(fmaf(s[i + 1], kLog2e, nm[r]));
+          l_run[r] += a0 + a1;
+          pa[kk][2 * h + r] = pack_bf16x2(a0, a1);
+        }
+    mbar_wait(&kv_full[st(2 * j + 1)], ph(2 * j + 1));
+    {
+      const uint32_t b = kv_addr + st(2 * j + 1) * T5_KV_BYTES;
+      wgmma_fence();
+#pragma unroll
+      for (int kk = 0; kk < T5_TK / 16; ++kk)
+        // V: 16 key rows of 128 B (all 64 head dims) per k-step
+        wgmma_rs<T5_D, true>(o, pa[kk], make_smem_desc(b + kk * 2048, 1024, 1024), 1);
+      wgmma_commit();
+      wgmma_wait<0>();
+      reg_fence(o);
+    }
+    if (leader) mbar_arrive(&kv_empty[st(2 * j + 1)]);
+  }
+#pragma unroll
+  for (int r = 0; r < 2; ++r) {
+    float l = l_run[r];
+    l += __shfl_xor_sync(0xffffffffu, l, 1);
+    l += __shfl_xor_sync(0xffffffffu, l, 2);
+    const float inv_l = 1.0f / l;
+    if (q_row[r] < p.L) {
+      uint16_t* orow = reinterpret_cast<uint16_t*>(p.out) + static_cast<size_t>(q_row[r]) * p.ldo + col + 2 * (lane & 3);
+#pragma unroll
+      for (int nb = 0; nb < T5_D / 8; ++nb)
+        *reinterpret_cast<uint32_t*>(orow + nb * 8) = pack_bf16x2(o[4 * nb + 2 * r] * inv_l, o[4 * nb + 2 * r + 1] * inv_l);
+    }
   }
 }
 

@@ -1,6 +1,6 @@
-// kr_vae.cu — causal 3D VAE decoder kernels for sm_100a (channels-last activations).
+// kr_vae.cu — causal 3D VAE decoder kernels for sm_90a (channels-last activations).
 //
-// conv3d_igemm : CausalConv3d / Conv2d / 1x1x1 conv as an implicit GEMM on tcgen05 + TMEM.
+// conv3d_igemm : CausalConv3d / Conv2d / 1x1x1 conv as an implicit GEMM on wgmma.
 //   Reference: wan/modules/vae.py:17-36 (CausalConv3d: cat(cache, x) on T, zero-pad H/W, cuDNN
 //   conv), :175-209 (ResidualBlock: RMS_norm -> SiLU -> conv, twice, + shortcut),
 //   demo_utils/vae_block3.py:46-91 (Resample), :386-443 (VAEDecoder3d).
@@ -11,7 +11,9 @@
 //   frame), N = Cout, K = taps * Cin; the A tile of tap (kt,kh,kw) is ONE 4-D TMA box
 //   {64 ch, TW, TH, 1} at (c0, w0+kw-1, h0+kh-1, t+kt) landing in the canonical K-major
 //   SWIZZLE_128B layout; weights are pre-permuted to [Cout, taps*Cin].
-//   Epilogue (thread = pixel, all Cout columns of its TMEM lane): bias, optional residual add,
+//   Two consumer warpgroups hold the fp32 accumulators of 64 pixels x Cout each in registers; a TMA
+//   warpgroup feeds the smem ring.  Epilogue (from the accumulator fragment: a pixel's channels are spread over
+//   the 4 lanes of a quad): bias, optional residual add,
 //   optional raw store, optional fused RMS_norm(channel) * sqrt(C) * gamma -> SiLU store
 //   (vae.py:39-54, :184-186) for the NEXT conv's input, or clamp -> fp32 NCHW pixels.
 // Small HBM-bound kernels: latent un-scaling + conv2 (vae_block3.py:205-214), RMS_norm+SiLU,
@@ -23,7 +25,7 @@
 
 namespace kr {
 
-static constexpr int kConvThreads = 192;
+static constexpr int kConvThreads = 384;   // consumer warpgroups 0, 1 + TMA warpgroup
 
 template <int CIN, int N>
 struct ConvCfg {
@@ -36,28 +38,12 @@ struct ConvCfg {
   static constexpr int kB32 = kHas32 ? N * 64 : 0;
   static constexpr int kStageBytes = kA64 + kA32 + kB64 + kB32;
   static constexpr int kStages = (200 * 1024) / kStageBytes > 8 ? 8 : (200 * 1024) / kStageBytes;
-  static constexpr int kMmaN = N > 256 ? N / 2 : N;
+  static constexpr int kMmaN = N > 256 ? N / 2 : N;              // wgmma N <= 256
   static constexpr int kMmaSplit = N / kMmaN;
-  static constexpr int kNumAcc = N > 256 ? 1 : 2;
-  static constexpr int kAccStride = N;                            // TMEM columns between buffers
-  static constexpr int kTmemCols = (kNumAcc * N) <= 32 ? 32 : (kNumAcc * N) <= 64 ? 64
-                                   : (kNumAcc * N) <= 128 ? 128 : (kNumAcc * N) <= 256 ? 256 : 512;
   static constexpr int kSmemBytes = kStages * kStageBytes + 1024 + 256;
   static_assert(kStages >= 2, "pipeline needs >= 2 stages");
   static_assert(kB64 % 1024 == 0 && (kB32 % 512) == 0, "swizzle alignment of B tiles");
 };
-
-
-KR_DEVICE void tmem_ld_x16(uint32_t taddr, uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]),
-        "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]),
-        "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-}
 
 template <bool kBf16>
 KR_DEVICE float rnd16(float x) {
@@ -78,150 +64,86 @@ KR_DEVICE float load16(const uint16_t* p) {
                : __half2float(*reinterpret_cast<__half*>(&u));
 }
 
-// Epilogue of one output pixel (thread = TMEM lane): bias, optional residual, rounding, raw store, fused
-// RMS_norm*sqrt(C)*gamma -> SiLU store, or clamp -> fp32 NCHW pixels (N == 16 head).  `t_row` is the TMEM
-// address of this thread's accumulator row; the accumulator is released on `empty_bar` (one arrive per warp)
-// as soon as its last column has been read.
+// Epilogue of the two output pixels of this thread's accumulator fragment (rows lane/4 and lane/4 + 8 of its
+// warp's 16; channel pairs 8*nb + 2*(lane%4)): bias, optional residual, rounding, raw store, fused
+// RMS_norm*sqrt(C)*gamma -> SiLU store (the sum of squares is reduced over the quad), or clamp -> fp32 NCHW
+// pixels (N == 16 head).
 template <int N, bool kBf16>
-KR_DEVICE void conv_epilogue_pixel(const ConvParams& p, uint32_t t_row, int t, int h, int w, uint64_t* empty_bar,
-                                   int lane) {
+KR_DEVICE void conv_epilogue_frag(const ConvParams& p, float (&acc)[N / 2], int t, const int (&hh)[2],
+                                  const int (&ww)[2], int lane) {
   const uint16_t* bias = reinterpret_cast<const uint16_t*>(p.bias);
   const uint16_t* gamma = reinterpret_cast<const uint16_t*>(p.gamma);
-  // sub2: stride-2 convolution with right/bottom zero pad (ZeroPad2d((0,1,0,1)) + Conv2d(stride 2),
-  // vae.py:84-92) evaluated as the stride-1 conv at the odd positions: out(i,j) = full(2i+1, 2j+1)
-  const bool ok = h < p.H && w < p.W && (p.sub2 == 0 || ((h & 1) && (w & 1)));
-  const long pix = p.sub2 ? static_cast<long>(h >> 1) * (p.W >> 1) + (w >> 1)
-                          : static_cast<long>(h) * p.W + w;
-
-  if constexpr (N == 16) {
-    // head conv: bias, round, clamp, fp32 NCHW pixels
-    uint32_t v[16];
-    tmem_ld_x16(t_row, v);
-    tmem_ld_wait();
-    tc_fence_before();
-    __syncwarp();
-    if (lane == 0) mbar_arrive(empty_bar);
-    if (ok) {
-      for (int c = 0; c < p.cout; ++c) {
-        float x = __uint_as_float(v[c]) + (bias ? load16<kBf16>(bias + c) : 0.f);
-        x = rnd16<kBf16>(x);
-        if (p.out_pix != nullptr) {
-          x = fminf(fmaxf(x, -1.f), 1.f);
-          p.out_pix[(static_cast<long>(t) * p.cout + c) * p.H * p.W + pix] = x;
-        }
-      }
-    }
-  } else {
-    const uint16_t* res = p.residual
-        ? reinterpret_cast<const uint16_t*>(p.residual) + t * p.res_frame + pix * p.res_pix : nullptr;
-    uint16_t* oraw = p.out_raw
-        ? reinterpret_cast<uint16_t*>(p.out_raw) + t * p.raw_frame + pix * p.raw_pix : nullptr;
-    uint16_t* onrm = p.out_norm
-        ? reinterpret_cast<uint16_t*>(p.out_norm) + t * p.norm_frame + pix * p.norm_pix : nullptr;
-    float sumsq = 0.f;
-    // ---- pass 1: bias (+ residual), round, raw store, sum of squares; keep v in TMEM ----
-#pragma unroll 1
-    for (int c = 0; c < N / 32; ++c) {
-      uint32_t v[32];
-      tmem_ld_x32(t_row + c * 32, v);
-      tmem_ld_wait();
-      if (c == N / 32 - 1 && p.out_norm == nullptr) {
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(empty_bar);
-      }
-      float f[32];
+  const int cq = 2 * (lane & 3);
 #pragma unroll
-      for (int i = 0; i < 32; ++i) f[i] = __uint_as_float(v[i]);
-      if (bias != nullptr) {
-        const uint4* b4 = reinterpret_cast<const uint4*>(bias + c * 32);
+  for (int r = 0; r < 2; ++r) {
+    const int h = hh[r], w = ww[r];
+    // sub2: stride-2 convolution with right/bottom zero pad (ZeroPad2d((0,1,0,1)) + Conv2d(stride 2),
+    // vae.py:84-92) evaluated as the stride-1 conv at the odd positions: out(i,j) = full(2i+1, 2j+1)
+    const bool ok = h < p.H && w < p.W && (p.sub2 == 0 || ((h & 1) && (w & 1)));
+    const long pix = p.sub2 ? static_cast<long>(h >> 1) * (p.W >> 1) + (w >> 1)
+                            : static_cast<long>(h) * p.W + w;
+    if constexpr (N == 16) {
+      // head conv: bias, round, clamp, fp32 NCHW pixels
+      if (ok && p.out_pix != nullptr) {
 #pragma unroll
-        for (int q = 0; q < 4; ++q) {
-          const uint4 bb = __ldg(b4 + q);
-          const uint32_t wv[4] = {bb.x, bb.y, bb.z, bb.w};
+        for (int nb = 0; nb < 2; ++nb)
 #pragma unroll
-          for (int hh = 0; hh < 4; ++hh) {
-            const float2 g = unpack16<kBf16>(wv[hh]);
-            f[q * 8 + hh * 2] += g.x;
-            f[q * 8 + hh * 2 + 1] += g.y;
-          }
-        }
-      }
-      if (res != nullptr && ok) {
-        // reference: y = conv(...) (rounded to 16-bit), out = x + y (rounded)
-        const uint4* r4 = reinterpret_cast<const uint4*>(res + c * 32);
-#pragma unroll
-        for (int q = 0; q < 4; ++q) {
-          const uint4 rr = r4[q];
-          const uint32_t wv[4] = {rr.x, rr.y, rr.z, rr.w};
-#pragma unroll
-          for (int hh = 0; hh < 4; ++hh) {
-            const float2 g = unpack16<kBf16>(wv[hh]);
-            f[q * 8 + hh * 2] = g.x + rnd16<kBf16>(f[q * 8 + hh * 2]);
-            f[q * 8 + hh * 2 + 1] = g.y + rnd16<kBf16>(f[q * 8 + hh * 2 + 1]);
-          }
-        }
-      }
-#pragma unroll
-      for (int i = 0; i < 32; ++i) {
-        f[i] = rnd16<kBf16>(f[i]);
-        sumsq += f[i] * f[i];
-      }
-      if (oraw != nullptr && ok) {
-#pragma unroll
-        for (int q = 0; q < 4; ++q) {
-          uint4 o;
-          o.x = pack16<kBf16>(f[q * 8 + 0], f[q * 8 + 1]);
-          o.y = pack16<kBf16>(f[q * 8 + 2], f[q * 8 + 3]);
-          o.z = pack16<kBf16>(f[q * 8 + 4], f[q * 8 + 5]);
-          o.w = pack16<kBf16>(f[q * 8 + 6], f[q * 8 + 7]);
-          reinterpret_cast<uint4*>(oraw + c * 32)[q] = o;
-        }
-      }
-      if (p.out_norm != nullptr) {
-#pragma unroll
-        for (int i = 0; i < 32; ++i) v[i] = __float_as_uint(f[i]);
-        tmem_st_x32(t_row + c * 32, v);
-      }
-    }
-    // ---- pass 2: F.normalize(x, dim=C) * sqrt(C) * gamma -> SiLU ----
-    if (p.out_norm != nullptr) {
-      tmem_st_wait();
-      const float nrm = rnd16<kBf16>(sqrtf(sumsq));
-      const float inv = 1.0f / fmaxf(nrm, 1e-30f);
-#pragma unroll 1
-      for (int c = 0; c < N / 32; ++c) {
-        uint32_t v[32];
-        tmem_ld_x32(t_row + c * 32, v);
-        tmem_ld_wait();
-        if (c == N / 32 - 1) {
-          tc_fence_before();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(empty_bar);
-        }
-        if (ok) {
-          const uint4* g4 = reinterpret_cast<const uint4*>(gamma + c * 32);
-#pragma unroll
-          for (int q = 0; q < 4; ++q) {
-            const uint4 gg = __ldg(g4 + q);
-            const uint32_t wv[4] = {gg.x, gg.y, gg.z, gg.w};
-            float o[8];
-#pragma unroll
-            for (int hh = 0; hh < 4; ++hh) {
-              const float2 g = unpack16<kBf16>(wv[hh]);
-              float a = rnd16<kBf16>(__uint_as_float(v[q * 8 + hh * 2]) * inv);
-              float b = rnd16<kBf16>(__uint_as_float(v[q * 8 + hh * 2 + 1]) * inv);
-              a = rnd16<kBf16>(rnd16<kBf16>(a * p.norm_scale) * g.x);
-              b = rnd16<kBf16>(rnd16<kBf16>(b * p.norm_scale) * g.y);
-              o[hh * 2] = a / (1.0f + __expf(-a));
-              o[hh * 2 + 1] = b / (1.0f + __expf(-b));
+          for (int e = 0; e < 2; ++e) {
+            const int c = nb * 8 + cq + e;
+            if (c < p.cout) {
+              float x = acc[4 * nb + 2 * r + e] + (bias ? load16<kBf16>(bias + c) : 0.f);
+              x = fminf(fmaxf(rnd16<kBf16>(x), -1.f), 1.f);
+              p.out_pix[(static_cast<long>(t) * p.cout + c) * p.H * p.W + pix] = x;
             }
-            uint4 ov;
-            ov.x = pack16<kBf16>(o[0], o[1]);
-            ov.y = pack16<kBf16>(o[2], o[3]);
-            ov.z = pack16<kBf16>(o[4], o[5]);
-            ov.w = pack16<kBf16>(o[6], o[7]);
-            reinterpret_cast<uint4*>(onrm + c * 32)[q] = ov;
+          }
+      }
+    } else {
+      const uint16_t* res = (p.residual && ok)
+          ? reinterpret_cast<const uint16_t*>(p.residual) + t * p.res_frame + pix * p.res_pix : nullptr;
+      uint16_t* oraw = (p.out_raw && ok)
+          ? reinterpret_cast<uint16_t*>(p.out_raw) + t * p.raw_frame + pix * p.raw_pix : nullptr;
+      float sumsq = 0.f;
+      // ---- pass 1: bias (+ residual), round, raw store, sum of squares ----
+#pragma unroll
+      for (int nb = 0; nb < N / 8; ++nb) {
+        const int c = nb * 8 + cq;
+        float f0 = acc[4 * nb + 2 * r], f1 = acc[4 * nb + 2 * r + 1];
+        if (bias != nullptr) {
+          const float2 g = unpack16<kBf16>(__ldg(reinterpret_cast<const unsigned int*>(bias + c)));
+          f0 += g.x;
+          f1 += g.y;
+        }
+        if (res != nullptr) {
+          // reference: y = conv(...) (rounded to 16-bit), out = x + y (rounded)
+          const float2 g = unpack16<kBf16>(*reinterpret_cast<const uint32_t*>(res + c));
+          f0 = g.x + rnd16<kBf16>(f0);
+          f1 = g.y + rnd16<kBf16>(f1);
+        }
+        f0 = rnd16<kBf16>(f0);
+        f1 = rnd16<kBf16>(f1);
+        sumsq += f0 * f0 + f1 * f1;
+        if (oraw != nullptr) *reinterpret_cast<uint32_t*>(oraw + c) = pack16<kBf16>(f0, f1);
+        acc[4 * nb + 2 * r] = f0;
+        acc[4 * nb + 2 * r + 1] = f1;
+      }
+      // ---- pass 2: F.normalize(x, dim=C) * sqrt(C) * gamma -> SiLU ----
+      if (p.out_norm != nullptr) {
+        sumsq += __shfl_xor_sync(0xffffffffu, sumsq, 1);
+        sumsq += __shfl_xor_sync(0xffffffffu, sumsq, 2);
+        const float nrm = rnd16<kBf16>(sqrtf(sumsq));
+        const float inv = 1.0f / fmaxf(nrm, 1e-30f);
+        if (ok) {
+          uint16_t* onrm = reinterpret_cast<uint16_t*>(p.out_norm) + t * p.norm_frame + pix * p.norm_pix;
+#pragma unroll
+          for (int nb = 0; nb < N / 8; ++nb) {
+            const int c = nb * 8 + cq;
+            const float2 g = unpack16<kBf16>(__ldg(reinterpret_cast<const unsigned int*>(gamma + c)));
+            float a = rnd16<kBf16>(acc[4 * nb + 2 * r] * inv);
+            float b = rnd16<kBf16>(acc[4 * nb + 2 * r + 1] * inv);
+            a = rnd16<kBf16>(rnd16<kBf16>(a * p.norm_scale) * g.x);
+            b = rnd16<kBf16>(rnd16<kBf16>(b * p.norm_scale) * g.y);
+            *reinterpret_cast<uint32_t*>(onrm + c) =
+                pack16<kBf16>(a / (1.0f + __expf(-a)), b / (1.0f + __expf(-b)));
           }
         }
       }
@@ -242,9 +164,6 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tm_in64, const __grid_cons
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + Cfg::kStages * Cfg::kStageBytes);
   uint64_t* full_bar = bars;
   uint64_t* empty_bar = bars + Cfg::kStages;
-  uint64_t* tmem_full = bars + 2 * Cfg::kStages;
-  uint64_t* tmem_empty = tmem_full + 2;
-  uint32_t* tmem_base_smem = reinterpret_cast<uint32_t*>(tmem_empty + 2);
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -255,37 +174,25 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tm_in64, const __grid_cons
   const int taps = p.KT * p.KH * p.KW;
   const int pad_h = p.KH / 2, pad_w = p.KW / 2;
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 256) {
     prefetch_tmap(&tm_in64);
     prefetch_tmap(&tm_w64);
     if (Cfg::kHas32) {
       prefetch_tmap(&tm_in32);
       prefetch_tmap(&tm_w32);
     }
-  }
-  if (warp == 1) {
-    if (lane == 0) {
-      for (int i = 0; i < Cfg::kStages; ++i) {
-        mbar_init(&full_bar[i], 1);
-        mbar_init(&empty_bar[i], 1);
-      }
-      for (int i = 0; i < 2; ++i) {
-        mbar_init(&tmem_full[i], 1);
-        mbar_init(&tmem_empty[i], 4);
-      }
-      fence_barrier_init();
+    for (int i = 0; i < Cfg::kStages; ++i) {
+      mbar_init(&full_bar[i], 1);
+      mbar_init(&empty_bar[i], 2);   // one arrive per consumer warpgroup
     }
-    __syncwarp();
-    tmem_alloc<Cfg::kTmemCols>(tmem_base_smem);
+    fence_barrier_init();
   }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_base_smem;
 
-  if (warp == 0) {
+  if (warp >= 8) {
     // ===================== TMA producer =====================
-    if (elect_one()) {
+    producer_regs();
+    if (warp == 8 && elect_one()) {
       int stage = 0;
       uint32_t phase = 0;
       for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
@@ -323,87 +230,66 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tm_in64, const __grid_cons
         }
       }
     }
-  } else if (warp == 1) {
-    // ===================== MMA issuer: ONE thread runs the whole loop =====================
-    if (elect_one()) {
-      constexpr uint32_t idesc = make_idesc<kBf16>(128, Cfg::kMmaN, 0, 0);
-      int stage = 0;
-      uint32_t phase = 0;
-      int acc = 0;
-      uint32_t acc_phase = 0;
-      const int k_stages = taps * Cfg::kStagesPerTap;
-      const uint32_t smem0 = smem_u32(smem);
-      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-        mbar_wait(&tmem_empty[acc], acc_phase ^ 1);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + acc * Cfg::kAccStride;
-        for (int ks = 0; ks < k_stages; ++ks) {
-          mbar_wait(&full_bar[stage], phase);
-          tc_fence_after();
-          const uint32_t st = smem0 + stage * Cfg::kStageBytes;
-          const uint32_t a64 = st, b64 = st + Cfg::kA64;
-#pragma unroll
-          for (int k = 0; k < 4; ++k) {
-            const uint64_t a_desc = make_smem_desc(a64 + k * 32, 16, 1024);
-#pragma unroll
-            for (int j = 0; j < Cfg::kMmaSplit; ++j) {
-              const uint64_t b_desc = make_smem_desc(b64 + j * Cfg::kMmaN * 128 + k * 32, 16, 1024);
-              umma_ss(d_tmem + j * Cfg::kMmaN, a_desc, b_desc, idesc, (ks | k) != 0 ? 1u : 0u);
-            }
-          }
-          if (Cfg::kHas32) {
-            const uint32_t a32 = st + Cfg::kA64 + Cfg::kB64, b32 = a32 + Cfg::kA32;
-#pragma unroll
-            for (int k = 0; k < 2; ++k) {
-              // SWIZZLE_64B: 64-byte rows, 8-row groups 512 B apart
-              const uint64_t a_desc = make_smem_desc(a32 + k * 32, 16, 512, 4);
-#pragma unroll
-              for (int j = 0; j < Cfg::kMmaSplit; ++j) {
-                const uint64_t b_desc = make_smem_desc(b32 + j * Cfg::kMmaN * 64 + k * 32, 16, 512, 4);
-                umma_ss(d_tmem + j * Cfg::kMmaN, a_desc, b_desc, idesc, 1u);
-              }
-            }
-          }
-          umma_commit(&empty_bar[stage]);
-          if (ks == k_stages - 1) umma_commit(&tmem_full[acc]);
-          if (++stage == Cfg::kStages) {
-            stage = 0;
-            phase ^= 1;
-          }
-        }
-        if (++acc == Cfg::kNumAcc) {
-          acc = 0;
-          acc_phase ^= 1;
-        }
-      }
-    }
-  } else {
-    // ===================== epilogue (thread = output pixel) =====================
-    const int quarter = warp & 3;
-    const int r = quarter * 32 + lane;          // row in tile
-    int acc = 0;
-    uint32_t acc_phase = 0;
-    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-      const int t = tile / tiles_per_frame;
-      const int rem = tile % tiles_per_frame;
-      const int h = (rem / tiles_w) * p.TH + r / p.TW;
-      const int w = (rem % tiles_w) * p.TW + r % p.TW;
-      mbar_wait(&tmem_full[acc], acc_phase);
-      tc_fence_after();
-      const uint32_t t_row = tmem_base + (static_cast<uint32_t>(quarter * 32) << 16) + acc * Cfg::kAccStride;
-      conv_epilogue_pixel<N, kBf16>(p, t_row, t, h, w, &tmem_empty[acc], lane);
-      if (++acc == Cfg::kNumAcc) {
-        acc = 0;
-        acc_phase ^= 1;
-      }
-    }
+    return;
   }
 
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc<Cfg::kTmemCols>(tmem_base);
+  // ===================== consumer warpgroups: wgmma over 64 pixels each, then the epilogue =====================
+  consumer_regs();
+  const int wg = warp >> 2;
+  const bool leader = (threadIdx.x & 127) == 0;
+  const int k_stages = taps * Cfg::kStagesPerTap;
+  const uint32_t smem0 = smem_u32(smem);
+  int stage = 0;
+  uint32_t phase = 0;
+  for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+    float acc[N / 2];
+    for (int ks = 0; ks < k_stages; ++ks) {
+      mbar_wait(&full_bar[stage], phase);
+      const uint32_t st = smem0 + stage * Cfg::kStageBytes;
+      const uint32_t a64 = st + wg * 64 * 128, b64 = st + Cfg::kA64;
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < 4; ++k) {
+        const uint64_t a_desc = make_smem_desc(a64 + k * 32, 16, 1024);
+#pragma unroll
+        for (int j = 0; j < Cfg::kMmaSplit; ++j) {
+          const uint64_t b_desc = make_smem_desc(b64 + j * Cfg::kMmaN * 128 + k * 32, 16, 1024);
+          wgmma_ss<Cfg::kMmaN, kBf16, 0>(acc + j * (Cfg::kMmaN / 2), a_desc, b_desc, (ks | k) != 0 ? 1 : 0);
+        }
+      }
+      if (Cfg::kHas32) {
+        const uint32_t a32 = st + Cfg::kA64 + Cfg::kB64 + wg * 64 * 64;
+        const uint32_t b32 = st + Cfg::kA64 + Cfg::kB64 + Cfg::kA32;
+#pragma unroll
+        for (int k = 0; k < 2; ++k) {
+          // SWIZZLE_64B: 64-byte rows, 8-row groups 512 B apart
+          const uint64_t a_desc = make_smem_desc(a32 + k * 32, 16, 512, kSwz64);
+#pragma unroll
+          for (int j = 0; j < Cfg::kMmaSplit; ++j) {
+            const uint64_t b_desc = make_smem_desc(b32 + j * Cfg::kMmaN * 64 + k * 32, 16, 512, kSwz64);
+            wgmma_ss<Cfg::kMmaN, kBf16, 0>(acc + j * (Cfg::kMmaN / 2), a_desc, b_desc, 1);
+          }
+        }
+      }
+      wgmma_commit();
+      wgmma_wait<0>();
+      reg_fence(acc);
+      if (leader) mbar_arrive(&empty_bar[stage]);
+      if (++stage == Cfg::kStages) {
+        stage = 0;
+        phase ^= 1;
+      }
+    }
+    const int t = tile / tiles_per_frame;
+    const int rem = tile % tiles_per_frame;
+    int hh[2], ww[2];
+#pragma unroll
+    for (int r = 0; r < 2; ++r) {
+      const int px = wg * 64 + (warp & 3) * 16 + (lane >> 2) + 8 * r;   // pixel row of the TH x TW tile
+      hh[r] = (rem / tiles_w) * p.TH + px / p.TW;
+      ww[r] = (rem % tiles_w) * p.TW + px % p.TW;
+    }
+    conv_epilogue_frag<N, kBf16>(p, acc, t, hh, ww, lane);
   }
 }
 
@@ -411,19 +297,20 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tm_in64, const __grid_cons
 // conv_halo_kernel: the 3x3-spatial convs of the wide stages (N = 96 / 192 output channels).
 //
 // conv_igemm_kernel fetches a fresh 128-pixel input tile AND a fresh weight tile for every one of the
-// kt*9 taps: ncu on the 96->96 stage-3 conv shows 44 GB of L2->SM traffic for 1.3 GB of input (12.9 TB/s,
-// the chip's L2->SM ceiling) and the tensor pipe at 34 %.  Here
+// kt*9 taps.  Here
 //   * one work item = 256 output pixels of one frame: two 16(h) x 8(w) MMA tiles side by side;
 //   * per (kt, 64-channel chunk) ONE halo box {64 ch, 24 w, 18 h} (18 x 24 = 432 rows of 128 B, pitch 24
-//     rows) is loaded, and the 9 spatial taps are MMAs over SHIFTED WINDOWS of it: the A descriptor of
-//     tap (kh, kw), tile u starts (kh*24 + 8u + kw) rows into the box with SBO = 24 rows.  The tensor core
-//     derives the 128-byte swizzle from absolute shared-memory address bits, so a start address that is
-//     not 1024-byte aligned needs no "base offset" (verified on B200: tools/experiments/umma_shift_test.cu,
-//     profiles/r01_umma_shifted_window_test.log);
-//   * every weight tile {64 k, N} is used by both pixel tiles (two accumulators in TMEM).
+//     rows) is loaded, and the 9 spatial taps are wgmmas over SHIFTED WINDOWS of it: a tile's pixel row
+//     (h, w) of tap (kh, kw) is box row (h + kh) * 24 + 8u + w + kw, so a 64-pixel slice is 8 groups of 8
+//     consecutive box rows, 24 rows (SBO = 3072 B, a multiple of the 1024 B swizzle atom) apart.  Only the
+//     start address is off the atom boundary (by kw rows); wgmma derives the 128-byte swizzle from the absolute
+//     shared-memory address bits, as TMA does when it writes the box, so the base-offset field stays 0;
+//   * every weight tile {64 k, N} is used by both pixel tiles.
 // Input traffic per pixel drops 9x * (128/216) and weight traffic 2x.  Borders are the TMA out-of-bounds
 // zero fill as before; a partial last channel chunk (CIN = 96) is loaded 64 wide (zero filled) and only
 // its valid k-steps are issued.
+// Consumer warpgroup u owns pixel tile u (two m64 halves, accumulators N registers per thread); warpgroup 2 is
+// the TMA producer.
 template <int CIN, int N>
 struct HaloCfg {
   static constexpr int kChunks = (CIN + 63) / 64;
@@ -433,12 +320,11 @@ struct HaloCfg {
   static constexpr int kAStages = 2;
   static constexpr int kBBytes = N * 128;
   static constexpr int kBStages = (96 * 1024) / kBBytes > 8 ? 8 : (96 * 1024) / kBBytes;
-  static constexpr int kAccSets = (4 * N <= 512) ? 2 : 1;        // double-buffer the accumulators if they fit
   static constexpr int kSmemBytes = kAStages * kABytes + kBStages * kBBytes + 1024 + 512;
   static_assert(kABytes % 1024 == 0 && kBBytes % 1024 == 0, "swizzle alignment");
-  static_assert(2 * N * kAccSets <= 512, "TMEM columns");
 };
-static constexpr int kHaloThreads = 64 + 256;   // TMA warp, MMA warp, 2 x 4 epilogue warps
+static constexpr int kHaloThreads = 384;
+
 
 template <int CIN, int N, bool kBf16>
 __global__ void __launch_bounds__(kHaloThreads, 1)
@@ -455,9 +341,6 @@ conv_halo_kernel(const __grid_constant__ CUtensorMap tm_in, const __grid_constan
   uint64_t* a_empty = a_full + Cfg::kAStages;      // [kAStages]
   uint64_t* b_full = a_empty + Cfg::kAStages;      // [kBStages]
   uint64_t* b_empty = b_full + Cfg::kBStages;      // [kBStages]
-  uint64_t* tmem_full = b_empty + Cfg::kBStages;   // [4] accumulator = set * 2 + tile
-  uint64_t* tmem_empty = tmem_full + 4;            // [4]
-  uint32_t* tmem_base_smem = reinterpret_cast<uint32_t*>(tmem_empty + 4);
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -466,37 +349,25 @@ conv_halo_kernel(const __grid_constant__ CUtensorMap tm_in, const __grid_constan
   const int items_per_frame = items_w * items_h;
   const int num_items = p.T * items_per_frame;
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 256) {
     prefetch_tmap(&tm_in);
     prefetch_tmap(&tm_w);
-  }
-  if (warp == 1) {
-    if (lane == 0) {
-      for (int i = 0; i < Cfg::kAStages; ++i) {
-        mbar_init(&a_full[i], 1);
-        mbar_init(&a_empty[i], 1);
-      }
-      for (int i = 0; i < Cfg::kBStages; ++i) {
-        mbar_init(&b_full[i], 1);
-        mbar_init(&b_empty[i], 1);
-      }
-      for (int i = 0; i < 4; ++i) {
-        mbar_init(&tmem_full[i], 1);
-        mbar_init(&tmem_empty[i], 4);   // one arrive per epilogue warp of the tile
-      }
-      fence_barrier_init();
+    for (int i = 0; i < Cfg::kAStages; ++i) {
+      mbar_init(&a_full[i], 1);
+      mbar_init(&a_empty[i], 2);
     }
-    __syncwarp();
-    tmem_alloc<512>(tmem_base_smem);
+    for (int i = 0; i < Cfg::kBStages; ++i) {
+      mbar_init(&b_full[i], 1);
+      mbar_init(&b_empty[i], 2);
+    }
+    fence_barrier_init();
   }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_base_smem;
 
-  if (warp == 0) {
+  if (warp >= 8) {
     // ===================== TMA producer =====================
-    if (elect_one()) {
+    producer_regs();
+    if (warp == 8 && elect_one()) {
       int sa = 0, sb = 0;
       uint32_t pa = 0, pb = 0;
       for (int item = blockIdx.x; item < num_items; item += gridDim.x) {
@@ -526,100 +397,73 @@ conv_halo_kernel(const __grid_constant__ CUtensorMap tm_in, const __grid_constan
         }
       }
     }
-  } else if (warp == 1) {
-    // ===================== MMA issuer (one thread) =====================
-    if (elect_one()) {
-      constexpr uint32_t idesc = make_idesc<kBf16>(128, N, 0, 0);
-      const uint64_t a_hi = make_smem_desc(0, 16, Cfg::kBoxW * 128) & 0xFFFFFFFF00000000ull;
-      const uint32_t a_lo_c = static_cast<uint32_t>(make_smem_desc(0, 16, Cfg::kBoxW * 128));
-      const uint64_t b_hi = make_smem_desc(0, 16, 1024) & 0xFFFFFFFF00000000ull;
-      const uint32_t b_lo_c = static_cast<uint32_t>(make_smem_desc(0, 16, 1024));
-      const uint32_t a0 = smem_u32(smem_a), b0 = smem_u32(smem_b);
-      int sa = 0, sb = 0;
-      uint32_t pa = 0, pb = 0;
-      int set = 0;
-      uint32_t set_phase = 0;
-      for (int item = blockIdx.x; item < num_items; item += gridDim.x) {
-        mbar_wait(&tmem_empty[set * 2 + 0], set_phase ^ 1);
-        mbar_wait(&tmem_empty[set * 2 + 1], set_phase ^ 1);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + set * 2 * N;
-        bool first = true;
-        for (int kt = 0; kt < p.KT; ++kt) {
-          for (int c = 0; c < Cfg::kChunks; ++c) {
-            const int ksteps = (c == Cfg::kChunks - 1) ? Cfg::kLastK : 4;
-            mbar_wait(&a_full[sa], pa);
-            tc_fence_after();
-            const uint32_t a_st = a0 + sa * Cfg::kABytes;
-#pragma unroll 1
-            for (int sp = 0; sp < 9; ++sp) {
-              const int kh = sp / 3, kw = sp - kh * 3;
-              mbar_wait(&b_full[sb], pb);
-              tc_fence_after();
-              const uint32_t b_st = b0 + sb * Cfg::kBBytes;
-              const uint32_t a_win = a_st + (kh * Cfg::kBoxW + kw) * 128;
-#pragma unroll
-              for (int u = 0; u < 2; ++u) {
-#pragma unroll
-                for (int k = 0; k < 4; ++k) {
-                  if (k < ksteps) {
-                    const uint64_t ad = a_hi | (a_lo_c + ((a_win + u * 8 * 128 + k * 32) >> 4));
-                    const uint64_t bd = b_hi | (b_lo_c + ((b_st + k * 32) >> 4));
-                    umma_ss(d_tmem + u * N, ad, bd, idesc, (first && k == 0) ? 0u : 1u);
-                  }
-                }
-              }
-              first = false;
-              umma_commit(&b_empty[sb]);
-              if (++sb == Cfg::kBStages) {
-                sb = 0;
-                pb ^= 1;
-              }
-            }
-            umma_commit(&a_empty[sa]);
-            if (++sa == Cfg::kAStages) {
-              sa = 0;
-              pa ^= 1;
-            }
-          }
-        }
-        umma_commit(&tmem_full[set * 2 + 0]);
-        umma_commit(&tmem_full[set * 2 + 1]);
-        if (++set == Cfg::kAccSets) {
-          set = 0;
-          set_phase ^= 1;
-        }
-      }
-    }
-  } else {
-    // ===================== epilogue: warps 2..5 -> tile 0, warps 6..9 -> tile 1 =====================
-    const int u = (warp - 2) >> 2;
-    const int quarter = warp & 3;               // TMEM lane quarter this warp may access
-    const int r = quarter * 32 + lane;          // pixel row of the 16 x 8 tile
-    int set = 0;
-    uint32_t set_phase = 0;
-    for (int item = blockIdx.x; item < num_items; item += gridDim.x) {
-      const int t = item / items_per_frame;
-      const int rem = item % items_per_frame;
-      const int h = (rem / items_w) * 16 + (r >> 3);
-      const int w = (rem % items_w) * 16 + u * 8 + (r & 7);
-      const int acc = set * 2 + u;
-      mbar_wait(&tmem_full[acc], set_phase);
-      tc_fence_after();
-      const uint32_t t_row = tmem_base + (static_cast<uint32_t>(quarter * 32) << 16) + acc * N;
-      conv_epilogue_pixel<N, kBf16>(p, t_row, t, h, w, &tmem_empty[acc], lane);
-      if (++set == Cfg::kAccSets) {
-        set = 0;
-        set_phase ^= 1;
-      }
-    }
+    return;
   }
 
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc<512>(tmem_base);
+  // ===================== consumer warpgroup u: pixel tile u of the item =====================
+  consumer_regs();
+  const int u = warp >> 2;
+  const bool leader = (threadIdx.x & 127) == 0;
+  const uint32_t a0 = smem_u32(smem_a), b0 = smem_u32(smem_b);
+  int sa = 0, sb = 0;
+  uint32_t pa = 0, pb = 0;
+  for (int item = blockIdx.x; item < num_items; item += gridDim.x) {
+    float acc[2][N / 2];      // m64 halves: tile rows h 0..7 and 8..15
+    bool first = true;
+    for (int kt = 0; kt < p.KT; ++kt) {
+      for (int c = 0; c < Cfg::kChunks; ++c) {
+        const int ksteps = (c == Cfg::kChunks - 1) ? Cfg::kLastK : 4;
+        mbar_wait(&a_full[sa], pa);
+        const uint32_t a_st = a0 + sa * Cfg::kABytes;
+#pragma unroll 1
+        for (int sp = 0; sp < 9; ++sp) {
+          const int kh = sp / 3, kw = sp - kh * 3;
+          mbar_wait(&b_full[sb], pb);
+          const uint32_t b_st = b0 + sb * Cfg::kBBytes;
+          const uint32_t a_win = a_st + (kh * Cfg::kBoxW + 8 * u + kw) * 128;
+          wgmma_fence();
+#pragma unroll
+          for (int k = 0; k < 4; ++k) {
+            if (k < ksteps) {
+              const uint64_t bd = make_smem_desc(b_st + k * 32, 16, 1024);
+#pragma unroll
+              for (int mh = 0; mh < 2; ++mh) {
+                const uint64_t ad = make_smem_desc(a_win + mh * 8 * Cfg::kBoxW * 128 + k * 32, 16, Cfg::kBoxW * 128);
+                wgmma_ss<N, kBf16, 0>(acc[mh], ad, bd, (first && k == 0) ? 0 : 1);
+              }
+            }
+          }
+          wgmma_commit();
+          wgmma_wait<0>();
+          reg_fence(acc[0]);
+          reg_fence(acc[1]);
+          first = false;
+          if (leader) mbar_arrive(&b_empty[sb]);
+          if (++sb == Cfg::kBStages) {
+            sb = 0;
+            pb ^= 1;
+          }
+        }
+        if (leader) mbar_arrive(&a_empty[sa]);
+        if (++sa == Cfg::kAStages) {
+          sa = 0;
+          pa ^= 1;
+        }
+      }
+    }
+    const int t = item / items_per_frame;
+    const int rem = item % items_per_frame;
+#pragma unroll
+    for (int mh = 0; mh < 2; ++mh) {
+      int hh[2], ww[2];
+#pragma unroll
+      for (int r = 0; r < 2; ++r) {
+        const int px = mh * 64 + (warp & 3) * 16 + (lane >> 2) + 8 * r;   // pixel row of the 16 x 8 tile
+        hh[r] = (rem / items_w) * 16 + (px >> 3);
+        ww[r] = (rem % items_w) * 16 + u * 8 + (px & 7);
+      }
+      conv_epilogue_frag<N, kBf16>(p, acc[mh], t, hh, ww, lane);
+    }
   }
 }
 

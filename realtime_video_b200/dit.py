@@ -1,4 +1,4 @@
-"""Causal Wan DiT on the B200 kernels — host-side mirror of the reference's model classes.
+"""Causal Wan DiT on the sm_90a kernels — host-side mirror of the reference's model classes.
 
 Mirrors ``wan/modules/causal_model.py`` (CausalWanModel :526, CausalWanAttentionBlock :400,
 CausalWanSelfAttention :174, CausalHead :495) and ``wan/modules/model.py``
@@ -31,7 +31,7 @@ from . import ops
 
 def _linear(x: torch.Tensor, lin: nn.Linear, **kw) -> torch.Tensor:
     """nn.Linear of a DiT block on the GEMM kernels: bf16 by default, FP8 (dynamic per-tensor activation cast +
-    kind::f8f6f4 GEMM) when ``realtime_video_b200.fp8.quantize_`` attached quantised weights to the module."""
+    e4m3 wgmma GEMM) when ``realtime_video_b200.fp8.quantize_`` attached quantised weights to the module."""
     q = getattr(lin, "_kr_fp8", None)
     if q is None:
         return ops.gemm(x, lin.weight, lin.bias, **kw)

@@ -1,4 +1,4 @@
-"""Drop-in boundary: make the reference's import names resolve to the B200 classes (SURVEY.md §8b).
+"""Drop-in boundary: make the reference's import names resolve to this package's classes (SURVEY.md §8b).
 
 The reference has no FFI; its callers (``release_server.py``, ``sample.py``, ``pipeline/causal_inference.py``)
 reach the hot path through four module names.  :func:`install` puts ONE finder in front of ``sys.meta_path``

@@ -1,5 +1,5 @@
 """``python -m realtime_video_b200.dropin <script.py | -m module> [args...]`` — run an unmodified reference entry
-point (sample.py, ``-m uvicorn release_server:app`` ...) with the B200 classes behind the reference's import names."""
+point (sample.py, ``-m uvicorn release_server:app`` ...) with this package's classes behind the reference's import names."""
 import runpy
 import sys
 

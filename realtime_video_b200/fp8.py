@@ -1,4 +1,4 @@
-"""FP8 (e4m3) DiT linears — the B200 counterpart of the reference's ``enable_fp8`` switch (release_server.py:179-182):
+"""FP8 (e4m3) DiT linears — this package's counterpart of the reference's ``enable_fp8`` switch (release_server.py:179-182):
 
     from torchao.quantization.quant_api import quantize_, Float8DynamicActivationFloat8WeightConfig, PerTensor
     quantize_(transformer, Float8DynamicActivationFloat8WeightConfig(granularity=PerTensor()))
@@ -7,7 +7,7 @@ torchao turns every ``nn.Linear`` into: per-tensor dynamic e4m3 cast of the inpu
 with its own per-tensor scale, ``torch._scaled_mm`` with fp32 accumulation and bf16 output.  :func:`quantize_` does the
 same to the drop-in transformer: it attaches ``(w_q bytes, scale_w)`` to the Linear modules of the DiT blocks and the
 block schedule (realtime_video_b200/dit.py ``_linear``) then runs ``kr_fp8_quantize`` + ``kr_gemm_fp8``
-(tcgen05.mma.kind::f8f6f4, the bf16 GEMM's fused epilogues).  The embedding / head linears (0.04 % of the FLOPs) stay
+(e4m3 wgmma, the bf16 GEMM's fused epilogues).  The embedding / head linears (0.04 % of the FLOPs) stay
 bf16.  ``realtime_video_b200.dropin`` serves this module as ``torchao.quantization.quant_api`` so the server's own three
 lines above work unchanged.
 

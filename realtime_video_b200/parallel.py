@@ -4,7 +4,7 @@ The hot path is ONE strictly sequential stream (B=1; every pass needs the previo
 into independent units.  Here all N GPUs of a box work on the same block:
 
   * token rows are sharded contiguously (L/N rows per rank) for everything token-wise: LayerNorm/modulation,
-    QKV / o / cross-attention / FFN GEMMs (stream-K kernel: an L/N-row GEMM has too few tiles for 148 SMs),
+    QKV / o / cross-attention / FFN GEMMs (stream-K kernel: an L/N-row GEMM has too few tiles for 132 SMs),
     RMSNorm+RoPE — weights replicated (28 GB of 180 GB);
   * self-attention is sharded by HEAD (heads/N per rank, full sequence).
 

@@ -1,4 +1,4 @@
-"""UMT5 text encoder (SURVEY.md §8f.3) on the sm_100a kernels: the reference's ``T5Encoder`` with
+"""UMT5 text encoder (SURVEY.md §8f.3) on the sm_90a kernels: the reference's ``T5Encoder`` with
 ``shared_pos=False`` (wan/modules/t5.py:267-313; umt5-xxl: dim 4096, 64 heads x 64, ffn 10240, 24 layers,
 32 relative-position buckets, :456-469).  Off the per-frame path — it runs once per prompt / prompt change
 (release_server.py:459-468, :642) — so the schedule favours reuse of the existing kernels over launch count:

@@ -1,4 +1,4 @@
-"""Causal 3D VAE decoder on the B200 kernels — host-side mirror of the reference's decoder.
+"""Causal 3D VAE decoder on the sm_90a kernels — host-side mirror of the reference's decoder.
 
 Mirrors ``demo_utils/vae_block3.py`` (VAEDecoderWrapper :177-230, VAEDecoder3d :334-443) and the
 layers of ``wan/modules/vae.py`` it is built from (CausalConv3d :17, RMS_norm :39, Resample :66,
@@ -247,7 +247,7 @@ class _StreamLedger:
 
 
 class DecoderEngine(_StreamLedger):
-    """Runs VAEDecoder3d (+ the wrapper's un-scale and conv2) on the sm_100a kernels."""
+    """Runs VAEDecoder3d (+ the wrapper's un-scale and conv2) on the sm_90a kernels."""
 
     MAX_CHUNK = 3          # latent frames per launch sequence
 
@@ -649,7 +649,7 @@ class Encoder3d(nn.Module):
 
 
 class EncoderEngine(_StreamLedger):
-    """Encoder3d + WanVAE_.conv1 + latent scaling on the sm_100a kernels, streaming like the reference
+    """Encoder3d + WanVAE_.conv1 + latent scaling on the sm_90a kernels, streaming like the reference
     (demo_utils/vae_block3.py:141-175 over wan/modules/vae.py:301-345): the first chunk is ONE pixel frame on
     an empty cache (every causal conv sees zero history, the downsample3d time_convs are skipped and only
     remember their input, vae.py:160-163), every later chunk is FOUR frames -> one latent frame (time_conv
@@ -880,7 +880,7 @@ class VAEEncoderWrapper(nn.Module):
     @torch.compiler.disable
     def forward(self, z: torch.Tensor, feat_cache, stream: bool = False):
         if z.shape[0] != 1:
-            raise NotImplementedError("B200 VAE encoder: batch size 1 (as every call site of the reference)")
+            raise NotImplementedError("VAE encoder: batch size 1 (as every call site of the reference)")
         if self._engine is None:
             self._engine = EncoderEngine(self.encoder, self.conv1, self.mean, self.std)
         eng = self._engine

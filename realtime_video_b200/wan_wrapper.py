@@ -1,8 +1,8 @@
-"""The reference's ``utils/wan_wrapper.py`` on the B200 kernels (the L2 boundary, SURVEY.md §8b).
+"""The reference's ``utils/wan_wrapper.py`` on the sm_90a kernels (the L2 boundary, SURVEY.md §8b).
 
 Same class names, constructor arguments, attributes and call conventions as
 utils/wan_wrapper.py:20-323; the DiT underneath is ``realtime_video_b200.dit.CausalWanModel``, the text
-encoder ``realtime_video_b200.t5.T5Encoder`` and the VAE ``realtime_video_b200.vae`` (hand-written sm_100a
+encoder ``realtime_video_b200.t5.T5Encoder`` and the VAE ``realtime_video_b200.vae`` (hand-written sm_90a
 kernels behind the C ABI).  ``realtime_video_b200.dropin.install()`` serves this module under the name
 ``utils.wan_wrapper``, so the reference's own ``pipeline/causal_inference.py`` and ``release_server.py``
 construct and call these classes unchanged.
@@ -349,7 +349,7 @@ class WanDiffusionWrapper(nn.Module):
 class WanVAEWrapper(nn.Module):
     """utils/wan_wrapper.py:58-118 — classic-path VAE.  ``self.model`` carries the reference's WanVAE_
     state-dict keys (``encoder.*``, ``conv1.*``, ``conv2.*``, ``decoder.*``); decode and encode run on the
-    sm_100a engines in the tensor's 16-bit dtype (bf16 on the classic path, wan_wrapper.py:102-104)."""
+    sm_90a engines in the tensor's 16-bit dtype (bf16 on the classic path, wan_wrapper.py:102-104)."""
 
     def __init__(self, load_pretrained: bool = True):
         """``load_pretrained=False`` (not in the reference) builds the module tree without

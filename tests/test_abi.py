@@ -65,14 +65,16 @@ def test_product_never_imports_the_oracle():
 
 
 def test_gemm_kernel_plan_for_the_bench_shapes():
-    """Host-only query: which kernel kr_gemm serves a shape with on a 148-SM part (the CPU box falls back to 148).
-    M = 4680 token rows: the wide projections go to the CTA-pair kernel, the N = 5120 shapes (380 pair tiles =
-    5.14 waves of 74 pairs) stay on the single-CTA kernel, small problems never use the pair kernel."""
+    """Host-only query: which kernel kr_gemm serves a shape with on a 132-SM part (the CPU box falls back to 132).
+    M = 4680 token rows: the 2-CTA cluster kernel is costed at its measured throughput (a pair-tile wave = 1.62
+    single-CTA waves), so every bench shape stays on the single-CTA kernels: the wide projections on the fixed width
+    (1), the N = 5120 ones (740 tiles = 5.6 waves of 256-wide tiles) and the prompt projection on the wave-fitted
+    width (4)."""
     from realtime_video_b200 import _lib
     lib = _lib.load()
-    assert lib.kr_gemm_kernel_id(0, 4680, 15360, 5120) == 2      # to_qkv
-    assert lib.kr_gemm_kernel_id(1, 4680, 13824, 5120) == 2      # ffn.0 + GELU
-    assert lib.kr_gemm_kernel_id(2, 4680, 5120, 5120) == 1       # o + gate/residual
-    assert lib.kr_gemm_kernel_id(2, 4680, 5120, 13824) == 1      # ffn.2 + gate/residual
-    assert lib.kr_gemm_kernel_id(0, 512, 10240, 4096) in (1, 4)  # prompt k/v: single-CTA family (fixed or wave-fitted width)
+    assert lib.kr_gemm_kernel_id(0, 4680, 15360, 5120) == 1      # to_qkv
+    assert lib.kr_gemm_kernel_id(1, 4680, 13824, 5120) == 1      # ffn.0 + GELU
+    assert lib.kr_gemm_kernel_id(2, 4680, 5120, 5120) == 4       # o + gate/residual
+    assert lib.kr_gemm_kernel_id(2, 4680, 5120, 13824) == 4      # ffn.2 + gate/residual
+    assert lib.kr_gemm_kernel_id(0, 512, 10240, 4096) == 4       # prompt k/v: wave-fitted width
     assert lib.kr_gemm_kernel_id(4, 4680, 15360, 5120) == 1      # fp32-output epilogue: single-CTA only

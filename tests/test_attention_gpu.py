@@ -1,4 +1,4 @@
-"""GPU parity of the tcgen05 attention kernel (kr_attn_fwd through the C ABI) against an fp32 torch
+"""GPU parity of the wgmma attention kernel (kr_attn_fwd through the C ABI) against an fp32 torch
 restatement of flash_attn_func / the FlexAttention block mask (wan/modules/attention.py:65-70,
 wan/modules/causal_model.py:134-138, 339-348).  Floating point, bf16 inputs: P is rounded to bf16 before
 P.V exactly like FlashAttention-2, so rel-L2 <= 1e-2 (observed 2.3e-3) and the tolerance is in the test.
@@ -58,7 +58,7 @@ def test_attention_matches_fp32_reference(Lq, Lkv, heads, block_len, window):
 @pytest.mark.parametrize("Lq", [100, 256, 384, 700])   # 100/384: last CTA of a head runs the single-tile mode
 def test_growing_scores_exercise_the_lazy_rescale(Lq):
     """Keys are scaled up along the sequence so the running row maximum jumps by far more than the
-    2^8 rescale threshold from one 128-key tile to the next: O is rescaled in TMEM while the previous
+    2^8 rescale threshold from one 128-key tile to the next: O is rescaled in registers while the previous
     tile's P.V must already have retired (the ordering the o_done barrier / issue order guarantee)."""
     from realtime_video_b200 import ops
     torch.manual_seed(5)

@@ -19,9 +19,9 @@ def fake_args(**kw):
 
 
 def fake_prof():
-    return {"gemm": {"flops": 5.6e14, "ms": 400.0, "n": 1246},
-            "gemm/gemm2_tn_kernel": {"flops": 2.8e14, "ms": 190.0, "n": 400},
-            "gemm/gemm_tn_kernel": {"flops": 2.8e14, "ms": 210.0, "n": 836},
+    return {"gemm": {"flops": 5.6e14, "ms": 800.0, "n": 1246},
+            "gemm/gemm_flex_kernel": {"flops": 2.8e14, "ms": 380.0, "n": 400},
+            "gemm/gemm_tn_kernel": {"flops": 2.8e14, "ms": 420.0, "n": 836},
             "attention": {"flops": 1.7e14, "ms": 190.0, "n": 400},
             "vae_conv": {"flops": 4.0e13, "ms": 44.0, "n": 73}}
 

@@ -82,7 +82,7 @@ def test_other_reference_modules_stay_importable(tmp_path):
             ('ref-misc', 'ref-vae', 'ref-tok', 'ref-memory', 'ref-scheduler')
         from pipeline import CausalInferencePipeline            # the reference's own class ...
         import realtime_video_b200.wan_wrapper as ww
-        assert CausalInferencePipeline.gen is ww.WanDiffusionWrapper      # ... built on the B200 wrapper
+        assert CausalInferencePipeline.gen is ww.WanDiffusionWrapper      # ... built on this package's wrapper
         assert ww.FlowMatchScheduler is FlowMatchScheduler      # the wrapper uses the reference's scheduler when it exists
         from demo_utils.vae import ZERO_VAE_CACHE, VAEDecoderWrapperSingle
         assert ZERO_VAE_CACHE == ['ref-cache']

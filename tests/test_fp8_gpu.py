@@ -1,7 +1,7 @@
-"""FP8 row (SURVEY.md 8f.4) on the B200, through the C ABI, against oracle/fp8_oracle.py (torchao's published
+"""FP8 row (SURVEY.md 8f.4) on the GPU, through the C ABI, against oracle/fp8_oracle.py (torchao's published
 per-tensor dynamic-activation algorithm; "parity unpinned": torchao is not in the image).
   * kr_fp8_quantize: e4m3 bytes and scale BIT-EXACT vs the oracle (same fp32 multiply, round-to-nearest-even cast);
-  * kr_gemm_fp8 (tcgen05.mma.kind::f8f6f4): products of e4m3 values are exact in fp32, only the accumulation order
+  * kr_gemm_fp8 (e4m3 wgmma, fp32 promotion per k-block): products of e4m3 values are exact in fp32, only the accumulation order
     differs -> rel-L2 <= 2e-3 on the bf16 output, every fused epilogue, the DiT shapes;
   * FP8 tier vs the bf16 path on one 14B-dim layer: rel-L2 <= 8e-2 (e4m3 has 3 mantissa bits; stated, not hidden)."""
 import pytest

@@ -78,8 +78,8 @@ def test_streamk_ragged_shapes(M, N, K):
 def test_plan_keeps_data_parallel_kernels_where_they_fill_the_machine():
     from realtime_video_b200 import _lib
     lib = _lib.load()
-    assert lib.kr_gemm_kernel_id_ws(0, 4680, 5120, 5120, 1) == 1        # 740 tiles = 5.0 waves
-    assert lib.kr_gemm_kernel_id_ws(0, 4680, 15360, 5120, 1) == 2       # CTA-pair kernel
+    assert lib.kr_gemm_kernel_id_ws(0, 4680, 5120, 5120, 1) == 4        # 740 tiles = 5.6 waves: wave-fitted width
+    assert lib.kr_gemm_kernel_id_ws(0, 4680, 15360, 5120, 1) == 1       # 2220 tiles = 16.8 waves: fixed-width kernel
     if os.environ.get("KR_GEMM_SK") == "1" and lib.kr_gemm_kernel_id_ws(0, 585, 5120, 5120, 1) == 3:
         pass                                                            # stream-K enabled in this process
     assert lib.kr_gemm_kernel_id_ws(0, 585, 5120, 5120, 0) in (1, 4)    # no workspace -> never stream-K (single-CTA family)

@@ -1,6 +1,6 @@
-"""Row a1 on the B200: the server's block loop (harness/server_loop.py — proven bit-equal to the unmodified
+"""Row a1 on the GPU: the server's block loop (harness/server_loop.py — proven bit-equal to the unmodified
 ``release_server.GenerationSession`` on the same drop-in classes by tests/test_reference_callers_cpu.py) on the
-sm_100a kernels, against ``tests/golden/server_loop_small.npz`` = the same loop executed by the reference's own
+sm_90a kernels, against ``tests/golden/server_loop_small.npz`` = the same loop executed by the reference's own
 modules (bf16 DiT, fp16 VAE; tests/golden/make_server_loop_golden.py).  4 blocks: cache init, recompute under the
 block-causal mask, 4 denoise passes with re-noising (recorded draws replayed), VAE decode, sliding context window,
 first-frame re-encode.  Tolerances: both sides round to bf16/fp16 at different points and the error compounds over

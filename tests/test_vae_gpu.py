@@ -1,4 +1,4 @@
-"""GPU parity: sm_100a VAE decoder (through the C ABI) vs golden outputs of the reference
+"""GPU parity: sm_90a VAE decoder (through the C ABI) vs golden outputs of the reference
 VAEDecoderWrapper and vs the CPU oracle.
 
 Tolerance (stated): the product path stores activations in fp16 (the server's VAE dtype,

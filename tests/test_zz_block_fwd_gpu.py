@@ -1,4 +1,4 @@
-"""kr_dit_block_fwd on the B200: one C-ABI call per DiT block must reproduce the per-op schedule BIT FOR BIT (it issues
+"""kr_dit_block_fwd on the GPU: one C-ABI call per DiT block must reproduce the per-op schedule BIT FOR BIT (it issues
 the same launches with the same arguments — tests/test_block_fwd_cpu.py proves that on the host; this is the live
 check), on the golden 2-layer model through cache, later-block and recompute passes, and on one 14B-width layer."""
 import pytest

@@ -1,4 +1,4 @@
-"""GPU bring-up checks for the raw kernels (run on the B200 box via gpurun).
+"""GPU bring-up checks for the raw kernels (run on a GPU box).
 
     python tools/bringup.py gemm|attn|elem|perf
 

@@ -1,4 +1,4 @@
-"""CTA-pair GEMM (kr_gemm2.cu) against torch fp32; run with KR_GEMM2=2 to force it on every shape."""
+"""2-CTA cluster GEMM (kr_gemm2.cu) against torch fp32; run with KR_GEMM2=2 to force it on every shape."""
 import math
 import sys
 

@@ -1,7 +1,7 @@
-"""Two library A/Bs on one B200 (short): (1) the VAE's two heavy 3x3x3 causal convs (S3: 96->96 at 480x832, S2: 192->192 at
+"""Two library A/Bs on one GPU (short): (1) the VAE's two heavy 3x3x3 causal convs (S3: 96->96 at 480x832, S2: 192->192 at
 240x416, 12 output frames, fp16) — ours (conv_halo_kernel incl. the fused RMS-norm/SiLU + residual epilogue) vs cuDNN
 through torch.nn.functional.conv3d (channels_last_3d, conv only, no epilogue); (2) FP8 GEMM — ours vs cuBLASLt
-(torch._scaled_mm) on the ffn.0 / ffn.2 shapes.    python tools/conv_fp8_ab.py > profiles/r02_conv_fp8_ab.log"""
+(torch._scaled_mm) on the ffn.0 / ffn.2 shapes.    python tools/conv_fp8_ab.py"""
 import sys
 
 import torch

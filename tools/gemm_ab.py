@@ -1,6 +1,6 @@
-"""GEMM A/B on one B200: ours (planned kernel, with and without the stream-K workspace) vs cuBLAS (torch F.linear)
+"""GEMM A/B on one GPU: ours (planned kernel, with and without the stream-K workspace) vs cuBLAS (torch F.linear)
 for the four DiT projections at M = 4680 and at the sequence-parallel shards M = 2340 / 1170 / 585.
-    python tools/gemm_ab.py > profiles/r02_gemm_ab.log"""
+    python tools/gemm_ab.py"""
 import sys
 
 import torch

@@ -1,7 +1,7 @@
 """Host time per DiT block with the kernel launchers stubbed out (no GPU needed): the per-op Python schedule (14 ctypes
 calls + temporaries) against ONE kr_dit_block_fwd call.  Builds the launch recorder of tests/kr_record_stubs.cu (the real
 kr_api.cu / kr_dit_block.cu / kr_host.cu linked against recording stand-ins) and times both paths on this machine's CPU.
-    python tools/host_overhead.py > profiles/r02_host_overhead.txt"""
+    python tools/host_overhead.py"""
 import ctypes
 import shutil
 import subprocess

@@ -1,6 +1,6 @@
 """Time the device JPEG egress (kr_frames_to_jpeg) on one 12-frame 832x480 block of decoder-like frames and the
 reference's host path (normalise + to_pil_image + Pillow save in a 24-thread pool, release_server.py:945-983) on
-the same frames.  Writes gpurun_out/jpeg_time.json."""
+the same frames.  Writes out/jpeg_time.json."""
 import io
 import json
 import os
@@ -68,8 +68,8 @@ def main():
            "host_cores": os.cpu_count(),
            "algorithmic_bytes": T * 3 * H * W * 4 + jpeg_bytes,
            "achieved_gbs": (T * 3 * H * W * 4 + jpeg_bytes) / (dev_ms * 1e-3) / 1e9}
-    Path(ROOT / "gpurun_out").mkdir(exist_ok=True)
-    (ROOT / "gpurun_out" / "jpeg_time.json").write_text(json.dumps(res))
+    Path(ROOT / "out").mkdir(exist_ok=True)
+    (ROOT / "out" / "jpeg_time.json").write_text(json.dumps(res))
     print(json.dumps(res))
 
 

@@ -1,5 +1,5 @@
-"""UMT5-XXL encoder (24 layers, dim 4096, 64 heads, ffn 10240, L = 512) on one B200: time per prompt, kernel split.
-    python tools/time_t5.py > profiles/r02_umt5_xxl_timing.log"""
+"""UMT5-XXL encoder (24 layers, dim 4096, 64 heads, ffn 10240, L = 512) on one GPU: time per prompt, kernel split.
+    python tools/time_t5.py"""
 import sys
 
 import torch
