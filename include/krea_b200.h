@@ -279,4 +279,9 @@ int kr_rgb8_to_jpeg(const unsigned char* rgb, int frames, int height, int width,
 #ifdef __cplusplus
 }
 #endif
+
+/* The quantised attention tier (kr_sage_quantize / kr_sage_attn) is declared in its own header: its entry points and
+ * kernels are one translation unit, kr_sage.cu, outside the API layer above. */
+#include "krea_b200_sage.h"
+
 #endif /* KREA_B200_H_ */

@@ -16,7 +16,7 @@ from pathlib import Path
 _PKG_DIR = Path(__file__).resolve().parent
 _CSRC = _PKG_DIR / "csrc"
 LIB_PATH = _PKG_DIR / "libkrea_b200.so"
-SOURCES = ["kr_host.cu", "kr_gemm.cu", "kr_gemm2.cu", "kr_gemm_sk.cu", "kr_gemm_fp8.cu", "kr_attn.cu", "kr_t5attn.cu", "kr_dit_elem.cu", "kr_vae.cu", "kr_jpeg.cu", "kr_dit_block.cu", "kr_api.cu"]
+SOURCES = ["kr_host.cu", "kr_gemm.cu", "kr_gemm2.cu", "kr_gemm_sk.cu", "kr_gemm_fp8.cu", "kr_attn.cu", "kr_sage.cu", "kr_t5attn.cu", "kr_dit_elem.cu", "kr_vae.cu", "kr_jpeg.cu", "kr_dit_block.cu", "kr_api.cu"]
 
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
@@ -47,7 +47,7 @@ def needs_build() -> bool:
         return True
     t = LIB_PATH.stat().st_mtime
     deps = list(_CSRC.glob("*.cu")) + list(_CSRC.glob("*.cuh")) + list(_CSRC.glob("*.h"))
-    deps.append(_PKG_DIR.parent / "include" / "krea_b200.h")
+    deps += list((_PKG_DIR.parent / "include").glob("*.h"))
     return any(d.exists() and d.stat().st_mtime > t for d in deps)
 
 
@@ -155,6 +155,12 @@ SIGNATURES = {
     "kr_rgb8_to_jpeg": [_vp, _i, _i, _i, _i, _vp, _l, _vp, _vp, _sz, _vp],
 }
 
+# the quantised attention tier (include/krea_b200_sage.h, kr_sage.cu); every function returns int
+SAGE_SIGNATURES = {
+    "kr_sage_quantize": [_vp, _i, _vp, _i, _vp, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp],
+    "kr_sage_attn": [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _f, _vp],
+}
+
 
 def load() -> ctypes.CDLL:
     """Load the shared library (building is the caller's job: ``__graft_entry__.build``)."""
@@ -181,7 +187,7 @@ def load() -> ctypes.CDLL:
         if hasattr(lib, "kr_jpeg_workspace_bytes"):
             lib.kr_jpeg_workspace_bytes.restype = _sz
             lib.kr_jpeg_workspace_bytes.argtypes = [_i, _i, _i]
-        for name, argtypes in SIGNATURES.items():
+        for name, argtypes in {**SIGNATURES, **SAGE_SIGNATURES}.items():
             fn = getattr(lib, name, None)
             if fn is None:
                 continue   # checked by tests/test_abi.py against the header

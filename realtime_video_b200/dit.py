@@ -191,6 +191,9 @@ class CausalWanModel(nn.Module):
         self.sp = None          # optional parallel.SequenceParallel (single-stream multi-GPU mode)
         self.pp = None          # optional parallel.LayerPipeline (layer-sharded multi-GPU mode, BASELINE configs[2])
         self.use_block_fwd = os.environ.get("KR_BLOCK_FWD", "0") not in ("", "0")   # one C-ABI call per block
+        # "sage": the cached self-attention and the cross-attention run on the INT8/FP8 quantised kernels (the
+        # reference's sageattention backend on H100); None: bf16 attention everywhere
+        self.attn_quant = "sage" if os.environ.get("KR_SAGE_ATTN", "0") not in ("", "0") else None
         self.init_weights()
         self.gradient_checkpointing = False
         self.block_mask = None
@@ -274,6 +277,14 @@ class CausalWanModel(nn.Module):
             raise RuntimeError(f"KV cache overflow: slot [{local_start}, {local_end}) of {kv_size}")
         return kc, vc, local_start, local_end, start_frame, current_end
 
+    def _unmasked_attention(self, q, k, v, heads: int, out=None):
+        """Attention without a mask (cache branch, cross-attention) on the tier ``attn_quant`` selects."""
+        if self.attn_quant is None:
+            return ops.attention(q, k, v, heads=heads, out=out)
+        if self.attn_quant == "sage":
+            return ops.sage_attention(q, k, v, heads=heads, out=out)
+        raise ValueError(f"attn_quant must be 'sage' or None, got {self.attn_quant!r}")
+
     def _self_attention(self, blk: CausalWanAttentionBlock, h, grid, kv_cache, current_start, mask):
         """causal_model.py:218-397: projections, q/k RMSNorm, RoPE, cache write, attention.
         The cache slot is resolved first so the fused QKV GEMM writes its V third straight into
@@ -317,7 +328,7 @@ class CausalWanModel(nn.Module):
             else:
                 max_att = sa._max_attention_frames * fs if sa.local_attn_size == -1 else sa.local_attn_size * fs
                 lo = max(0, local_end - max_att)
-                ops.attention(q_full, kc[lo:local_end], vc[lo:local_end], heads=heads, out=o_heads)
+                self._unmasked_attention(q_full, kc[lo:local_end], vc[lo:local_end], heads, out=o_heads)
             ops.comm_scatter_rows(o_heads, sp.peer_ptrs(o_rows[:, sp.rank * Dh:]), D, n_loc, sp.world)
             sp.barrier()
             return o_rows
@@ -350,7 +361,7 @@ class CausalWanModel(nn.Module):
             else:
                 max_att = sa._max_attention_frames * fs if sa.local_attn_size == -1 else sa.local_attn_size * fs
                 lo = max(0, local_end - max_att)
-                o = ops.attention(q_full, kc[lo:local_end], vc[lo:local_end], heads=heads)
+                o = self._unmasked_attention(q_full, kc[lo:local_end], vc[lo:local_end], heads)
             return sp.heads_to_rows(o)
         if sa.fused_projections and (2 * D) % 256 == 0:
             qk = torch.empty(L, 2 * D, dtype=h.dtype, device=h.device)
@@ -376,7 +387,7 @@ class CausalWanModel(nn.Module):
                                  window=mask.window, pad_keys=pad)
         max_att = sa._max_attention_frames * fs if sa.local_attn_size == -1 else sa.local_attn_size * fs
         lo = max(0, local_end - max_att)
-        return ops.attention(rq, kc[lo:local_end], vc[lo:local_end], heads=sa.num_heads)
+        return self._unmasked_attention(rq, kc[lo:local_end], vc[lo:local_end], sa.num_heads)
 
     def _cross_attention(self, blk: CausalWanAttentionBlock, h, ctx, cache):
         """wan/modules/model.py:171-228 (K/V of the prompt computed once, cached by assignment)."""
@@ -395,7 +406,7 @@ class CausalWanModel(nn.Module):
             if cache is not None:
                 cache["is_init"] = True
                 cache["k"], cache["v"] = k, v
-        return ops.attention(q, k[0].reshape(-1, D), v[0].reshape(-1, D), heads=ca.num_heads)
+        return self._unmasked_attention(q, k[0].reshape(-1, D), v[0].reshape(-1, D), ca.num_heads)
 
     # -- whole block as ONE C-ABI call (kr_dit_block_fwd) ---------------------------------------------------------
     # Opt-in (KR_BLOCK_FWD=1 or ``model.use_block_fwd = True``): the C function issues exactly the launches of the
@@ -403,7 +414,7 @@ class CausalWanModel(nn.Module):
     # is the host side — one ctypes crossing per block instead of 14 and no temporary tensors.
     def _block_fwd_eligible(self, blk: CausalWanAttentionBlock, x, crossattn_cache) -> bool:
         sa, ca = blk.self_attn, blk.cross_attn
-        return (self.sp is None and x.dtype == torch.bfloat16 and sa.fused_projections and (2 * self.dim) % 256 == 0
+        return (self.sp is None and self.attn_quant is None and x.dtype == torch.bfloat16 and sa.fused_projections and (2 * self.dim) % 256 == 0
                 and sa.qk_norm and ca.qk_norm and crossattn_cache is not None and bool(crossattn_cache["is_init"])
                 and getattr(ops, "_prof", None) is None
                 # not inside a CUDA-graph capture: the scratch workspace is cached across calls and must not come from
