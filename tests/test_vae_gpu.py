@@ -9,6 +9,7 @@ import pytest
 import torch
 
 from oracle.vae_oracle import synthetic_vae_params
+from tests import kernel_refs as R
 from tests.golden_io import load_npz, rel_l2
 
 pytestmark = pytest.mark.gpu
@@ -76,6 +77,30 @@ def test_conv_kernel_vs_torch_conv3d():
                      tile=_tile_for(H, W), out_raw=out)
         r = rel_l2(out, ref)
         assert r < 2e-3, f"conv {cin}->{cout} taps {taps}: rel_l2={r:.3e}"
+        if c.n != cout:
+            continue
+        # fused epilogue: out_raw = r16(res + r16(conv + bias)), out_norm = SiLU(RMS_norm(out_raw) * sqrt(C) * gamma).
+        # The conv sum differs from fp32 torch only in its order (<= 1 ulp of r16(conv)); the norm is checked on the
+        # kernel's own raw output, so it must match the rounded restatement to 1 ulp with few non-identical elements.
+        res = torch.randn(T, H, W, cout, device="cuda").half()
+        gam = (1 + 0.3 * torch.randn(cout, device="cuda")).half()
+        raw2 = torch.empty(T, H, W, cout, dtype=torch.float16, device="cuda")
+        nrm = torch.empty_like(raw2)
+        ops.vae_conv(x.cuda().contiguous(), c.weight, c.bias, n=c.n, cout=c.cout, T=T, taps=taps,
+                     tile=_tile_for(H, W), out_raw=raw2, out_norm=nrm, gamma=gam, residual=res)
+        y = R.r16(ref.double().cuda(), torch.float16)
+        want = R.r16(res.double() + y, torch.float16)
+        d = (raw2.double() - want).abs()
+        assert bool((d <= R.ulp(y, torch.float16) + R.ulp(want, torch.float16)).all()), (cin, cout, taps)
+        frac = float((d != 0).double().mean())
+        assert frac <= 2e-2, (cin, cout, taps, frac)
+        nref, _ = R.vae_rmsnorm_silu(raw2, gam, torch.float16)
+        dn = (nrm.double() - nref).abs()
+        worst_n = float((dn / R.ulp(nref, torch.float16)).max())
+        frac_n = float((dn != 0).double().mean())
+        assert worst_n <= 1 and frac_n <= 2e-2, (cin, cout, taps, worst_n, frac_n)
+        print(f"conv {cin}->{cout} taps {taps}: residual {frac:.2e} not identical; norm {worst_n:.2f} ulp, "
+              f"{frac_n:.2e} not identical")
 
 
 def test_single_frame_wrapper_vs_reference_golden():
