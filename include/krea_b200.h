@@ -87,6 +87,27 @@ int kr_gemm_fp8(int epilogue, const void* a, int lda, const void* w, int ldw, co
                 const void* gate, int gate_stride, int rows_per_gate, void* out2, int ldc2, int n_split, int row_offset,
                 void* stream);
 
+/* Row-scaled FP8 = torchao Float8DynamicActivationFloat8WeightConfig(granularity=PerRow()): one scale per activation
+ * row (token) and one per weight output channel, so one outlier sets the scale of its own row only.
+ *   kr_fp8_quantize_rows : x [rows, cols] bf16 -> q e4m3 bytes [rows, ldq], q[r] = sat(x[r] * 448 / amax_r) with
+ *                          amax_r = max(max|x[r]|, 1e-12) (round to nearest even); scale_rows [rows] fp32 receives
+ *                          amax_r / 448.  One read, one write; cols % 8 == 0, cols <= 14336.
+ *   kr_ln_modulate_fp8   : kr_ln_modulate whose bf16 output row is also cast like kr_fp8_quantize_rows into q /
+ *                          scale_rows (bit-identical to quantising kr_ln_modulate's output); out may be NULL, then
+ *                          only the e4m3 bytes and scales are written.
+ *   kr_gemm_fp8_rowwise  : kr_gemm_fp8 with scale_a -> [M] fp32 row scales and scale_w -> [N] fp32 channel scales
+ *                          (16-byte aligned): out = epilogue((a_q @ w_q^T) * scale_a[m] * scale_w[n] + bias). */
+int kr_fp8_quantize_rows(const void* x, int ldx, int rows, int cols, void* q, int ldq, float* scale_rows,
+                         void* stream);
+int kr_ln_modulate_fp8(const void* x, int ldx, void* out, int ldo, int rows, int D, float eps,
+                       const void* w, const void* b, const void* mod, int mod_rows, int shift_idx,
+                       int scale_idx, int rows_per_frame, int row_offset, void* q, int ldq, float* scale_rows,
+                       void* stream);
+int kr_gemm_fp8_rowwise(int epilogue, const void* a, int lda, const void* w, int ldw, const float* scale_a,
+                        const float* scale_w, const void* bias, void* out, int ldc, int M, int N, int K,
+                        const void* residual, int ldr, const void* gate, int gate_stride, int rows_per_gate, void* out2,
+                        int ldc2, int n_split, int row_offset, void* stream);
+
 /* Which kernel kr_gemm launches for this epilogue and shape: 1 = the single-CTA kernel, 2 = the 2-CTA
  * cluster kernel (128x256 tile per CTA, W multicast to both), 3 = the stream-K kernel (only with a workspace), 4 = the
  * single-CTA kernel with a runtime tile width fitted to whole waves of SMs (small-M shards).  Host-only

@@ -66,6 +66,46 @@ int kr_gemm_fp8(int epilogue, const void* a, int lda, const void* w, int ldw, co
   return kr::gemm_fp8_tn(epilogue, a, lda, w, ldw, p, scale_a, scale_w, static_cast<cudaStream_t>(stream));
 }
 
+#define KR_REQUIRE_LINKED(fn)                                                      \
+  do {                                                                             \
+    if (&kr::fn == nullptr) {                                                      \
+      kr::set_last_error("%s: kr::" #fn " is not linked into this build", __func__); \
+      return KR_ERR_CUDA;                                                          \
+    }                                                                              \
+  } while (0)
+
+int kr_fp8_quantize_rows(const void* x, int ldx, int rows, int cols, void* q, int ldq, float* scale_rows,
+                         void* stream) {
+  KR_REQUIRE(x && q && scale_rows, "null x/q/scale_rows");
+  KR_REQUIRE_LINKED(fp8_quantize_rows);
+  return kr::fp8_quantize_rows(x, ldx, rows, cols, q, ldq, scale_rows, static_cast<cudaStream_t>(stream));
+}
+
+int kr_ln_modulate_fp8(const void* x, int ldx, void* out, int ldo, int rows, int D, float eps,
+                       const void* w, const void* b, const void* mod, int mod_rows, int shift_idx,
+                       int scale_idx, int rows_per_frame, int row_offset, void* q, int ldq, float* scale_rows,
+                       void* stream) {
+  KR_REQUIRE(x && q && scale_rows, "null x/q/scale_rows");
+  KR_REQUIRE_LINKED(ln_modulate_fp8);
+  return kr::ln_modulate_fp8(x, ldx, out, ldo, rows, D, eps, w, b, mod, mod_rows, shift_idx, scale_idx,
+                             rows_per_frame, row_offset, q, ldq, scale_rows, static_cast<cudaStream_t>(stream));
+}
+
+int kr_gemm_fp8_rowwise(int epilogue, const void* a, int lda, const void* w, int ldw, const float* scale_a,
+                        const float* scale_w, const void* bias, void* out, int ldc, int M, int N, int K,
+                        const void* residual, int ldr, const void* gate, int gate_stride, int rows_per_gate, void* out2,
+                        int ldc2, int n_split, int row_offset, void* stream) {
+  KR_REQUIRE(a && w && out, "null a/w/out");
+  KR_REQUIRE(scale_a && scale_w, "null scale_a/scale_w");
+  KR_REQUIRE_LINKED(gemm_fp8_rowwise_tn);
+  kr::GemmParams p;
+  p.out = out; p.bias = bias; p.residual = residual; p.gate = gate;
+  p.M = M; p.N = N; p.K = K; p.ldc = ldc; p.ldr = ldr; p.gate_stride = gate_stride;
+  p.rows_per_gate = rows_per_gate; p.alpha = 1.0f;
+  p.out2 = out2; p.ldc2 = ldc2; p.n_split = n_split; p.row_offset = row_offset;
+  return kr::gemm_fp8_rowwise_tn(epilogue, a, lda, w, ldw, p, scale_a, scale_w, static_cast<cudaStream_t>(stream));
+}
+
 int kr_attn_fwd(int dtype, const void* q, int ldq, const void* k, int ldk, const void* v, int ldv,
                 void* out, int ldo, int Lq, int Lkv, int heads, float softmax_scale, int mask_mode,
                 int block_len, int window, int pad_keys, void* stream) {

@@ -15,6 +15,8 @@
 #include "kr_common.cuh"
 #include "kr_ops.h"
 
+#include <cuda_fp8.h>
+
 namespace kr {
 
 static constexpr int kRowThreads = 128;
@@ -32,6 +34,17 @@ KR_DEVICE float block_sum(float v, float* red) {
   if ((threadIdx.x & 31) == 0) red[w] = v;
   __syncthreads();
   float t = red[0] + red[1] + red[2] + red[3];
+  __syncthreads();
+  return t;
+}
+// block-wide max over kRowThreads threads (same slot rules as block_sum)
+KR_DEVICE float block_max(float v, float* red) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, o));
+  const int w = threadIdx.x >> 5;
+  if ((threadIdx.x & 31) == 0) red[w] = v;
+  __syncthreads();
+  float t = fmaxf(fmaxf(red[0], red[1]), fmaxf(red[2], red[3]));
   __syncthreads();
   return t;
 }
@@ -56,15 +69,58 @@ KR_DEVICE void store8(uint16_t* p, const float (&f)[8]) {
 //   y = bf16(LN(x) [* w + b])                       (torch layer_norm: one rounding)
 //   out = bf16(bf16(y * bf16(1 + scale)) + shift)   when mod != nullptr
 // mod layout: [frames, mod_rows, D]; scale = row `scale_idx`, shift = row `shift_idx`.
+// kFp8: the bf16 output row is also quantised per row to e4m3 (fp8_quantize_row below) for the row-scaled FP8 GEMM;
+// the bf16 store happens only when `out` is given.
 // ---------------------------------------------------------------------------
 // Row data stays PACKED (uint4 = 8 x bf16) in registers and is unpacked per pass: ~3x fewer live
 // registers than keeping floats -> more resident CTAs -> more bytes in flight per SM.
+
+// Dynamic per-row e4m3 cast of one row held packed in registers by a kRowThreads CTA (torchao PerRow):
+//   amax = max(max|x|, 1e-12), q = sat_e4m3(x * (448 / amax)) (round to nearest even), scale_out = amax / 448.
+// `red` holds 4 floats; every thread of the CTA must call it.
 template <int kVec>
-__global__ void __launch_bounds__(kRowThreads, 8)
-ln_modulate_kernel(const uint16_t* __restrict__ x, int ldx, uint16_t* __restrict__ out, int ldo,
-                   int D, float eps, const uint16_t* __restrict__ w, const uint16_t* __restrict__ b,
-                   const uint16_t* __restrict__ mod, int mod_rows, int shift_idx, int scale_idx,
-                   int rows_per_frame, int row_offset) {
+KR_DEVICE void fp8_quantize_row(const uint4 (&raw)[kVec], int nvec, float* red, uint8_t* __restrict__ qrow,
+                                float* __restrict__ scale_out) {
+  float m = 0.f;
+#pragma unroll
+  for (int i = 0; i < kVec; ++i) {
+    const int vi = threadIdx.x + i * kRowThreads;
+    if (vi < nvec) {
+      const uint32_t u[4] = {raw[i].x, raw[i].y, raw[i].z, raw[i].w};
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        const float2 f = unpack_bf16x2(u[j]);
+        m = fmaxf(m, fmaxf(fabsf(f.x), fabsf(f.y)));
+      }
+    }
+  }
+  const float amax = fmaxf(block_max(m, red), 1e-12f);
+  const float mul = 448.0f / amax;
+  if (threadIdx.x == 0) *scale_out = amax / 448.0f;
+#pragma unroll
+  for (int i = 0; i < kVec; ++i) {
+    const int vi = threadIdx.x + i * kRowThreads;
+    if (vi < nvec) {
+      const uint32_t u[4] = {raw[i].x, raw[i].y, raw[i].z, raw[i].w};
+      uint32_t o[2];
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        const float2 f = unpack_bf16x2(u[j]);
+        const uint32_t h = __nv_cvt_float2_to_fp8x2(make_float2(f.x * mul, f.y * mul), __NV_SATFINITE, __NV_E4M3);
+        if (j & 1) o[j >> 1] |= h << 16;
+        else o[j >> 1] = h;
+      }
+      *reinterpret_cast<uint2*>(qrow + vi * 8) = make_uint2(o[0], o[1]);
+    }
+  }
+}
+
+template <int kVec, bool kFp8>
+KR_DEVICE void ln_modulate_row(const uint16_t* __restrict__ x, int ldx, uint16_t* __restrict__ out, int ldo,
+                               int D, float eps, const uint16_t* __restrict__ w, const uint16_t* __restrict__ b,
+                               const uint16_t* __restrict__ mod, int mod_rows, int shift_idx, int scale_idx,
+                               int rows_per_frame, int row_offset, uint8_t* __restrict__ q, int ldq,
+                               float* __restrict__ scale_rows) {
   __shared__ float red[4];
   const int row = blockIdx.x;
   const uint16_t* xr = x + static_cast<size_t>(row) * ldx;
@@ -99,7 +155,7 @@ ln_modulate_kernel(const uint16_t* __restrict__ x, int ldx, uint16_t* __restrict
   const float rstd = rsqrtf(block_sum(ss, red) / D + eps);
   const uint16_t* mrow = nullptr;
   if (mod != nullptr) mrow = mod + static_cast<size_t>((row + row_offset) / rows_per_frame) * mod_rows * D;
-  uint16_t* orow = out + static_cast<size_t>(row) * ldo;
+  uint16_t* orow = kFp8 && out == nullptr ? nullptr : out + static_cast<size_t>(row) * ldo;
 #pragma unroll
   for (int i = 0; i < kVec; ++i) {
     const int vi = threadIdx.x + i * kRowThreads;
@@ -128,26 +184,71 @@ ln_modulate_kernel(const uint16_t* __restrict__ x, int ldx, uint16_t* __restrict
 #pragma unroll
         for (int j = 0; j < 8; ++j) y[j] = bf16_round(y[j] * bf16_round(1.0f + sc[j])) + sh[j];
       }
-      store8(orow + vi * 8, y);
+      if constexpr (kFp8) {
+        // the bf16 output row replaces the input in registers; it is quantised once the whole row is known
+        raw[i] = make_uint4(pack_bf16x2(y[0], y[1]), pack_bf16x2(y[2], y[3]), pack_bf16x2(y[4], y[5]),
+                            pack_bf16x2(y[6], y[7]));
+        if (orow != nullptr) *reinterpret_cast<uint4*>(orow + vi * 8) = raw[i];
+      } else {
+        store8(orow + vi * 8, y);
+      }
     }
   }
+  if constexpr (kFp8) fp8_quantize_row<kVec>(raw, nvec, red, q + static_cast<size_t>(row) * ldq, scale_rows + row);
+}
+
+template <int kVec>
+__global__ void __launch_bounds__(kRowThreads, 8)
+ln_modulate_kernel(const uint16_t* __restrict__ x, int ldx, uint16_t* __restrict__ out, int ldo,
+                   int D, float eps, const uint16_t* __restrict__ w, const uint16_t* __restrict__ b,
+                   const uint16_t* __restrict__ mod, int mod_rows, int shift_idx, int scale_idx,
+                   int rows_per_frame, int row_offset) {
+  ln_modulate_row<kVec, false>(x, ldx, out, ldo, D, eps, w, b, mod, mod_rows, shift_idx, scale_idx, rows_per_frame,
+                               row_offset, nullptr, 0, nullptr);
+}
+
+template <int kVec>
+__global__ void __launch_bounds__(kRowThreads, 8)
+ln_modulate_fp8_kernel(const uint16_t* __restrict__ x, int ldx, uint16_t* __restrict__ out, int ldo,
+                       int D, float eps, const uint16_t* __restrict__ w, const uint16_t* __restrict__ b,
+                       const uint16_t* __restrict__ mod, int mod_rows, int shift_idx, int scale_idx,
+                       int rows_per_frame, int row_offset, uint8_t* __restrict__ q, int ldq,
+                       float* __restrict__ scale_rows) {
+  ln_modulate_row<kVec, true>(x, ldx, out, ldo, D, eps, w, b, mod, mod_rows, shift_idx, scale_idx, rows_per_frame,
+                              row_offset, q, ldq, scale_rows);
+}
+
+static int ln_check(const char* who, int rows, int D, int ldx, int ldo, const void* w, const void* b, const void* mod,
+                    int rows_per_frame) {
+  if (D % 8 != 0 || D > kRowThreads * 8 * kMaxVec || rows <= 0 || ldx % 8 != 0 || ldo % 8 != 0) {
+    set_last_error("%s: unsupported D=%d rows=%d", who, D, rows);
+    return KR_ERR_UNSUPPORTED_SHAPE;
+  }
+  if ((w == nullptr) != (b == nullptr)) {
+    set_last_error("%s: weight and bias must both be given or both be null", who);
+    return KR_ERR_INVALID_ARG;
+  }
+  if (mod != nullptr && rows_per_frame <= 0) {
+    set_last_error("%s: rows_per_frame must be positive", who);
+    return KR_ERR_INVALID_ARG;
+  }
+  return KR_OK;
+}
+
+static int launch_status(const char* who) {
+  cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) {
+    set_last_error("%s: launch failed: %s", who, cudaGetErrorString(e));
+    return KR_ERR_CUDA;
+  }
+  return KR_OK;
 }
 
 int ln_modulate(const void* x, int ldx, void* out, int ldo, int rows, int D, float eps,
                 const void* w, const void* b, const void* mod, int mod_rows, int shift_idx,
                 int scale_idx, int rows_per_frame, int row_offset, cudaStream_t stream) {
-  if (D % 8 != 0 || D > kRowThreads * 8 * kMaxVec || rows <= 0 || ldx % 8 != 0 || ldo % 8 != 0) {
-    set_last_error("ln_modulate: unsupported D=%d rows=%d", D, rows);
-    return KR_ERR_UNSUPPORTED_SHAPE;
-  }
-  if ((w == nullptr) != (b == nullptr)) {
-    set_last_error("ln_modulate: weight and bias must both be given or both be null");
-    return KR_ERR_INVALID_ARG;
-  }
-  if (mod != nullptr && rows_per_frame <= 0) {
-    set_last_error("ln_modulate: rows_per_frame must be positive");
-    return KR_ERR_INVALID_ARG;
-  }
+  const int rc = ln_check("ln_modulate", rows, D, ldx, ldo, w, b, mod, rows_per_frame);
+  if (rc != KR_OK) return rc;
   const int nv = (D / 8 + kRowThreads - 1) / kRowThreads;
 #define KR_LN_LAUNCH(V)                                                                            \
   ln_modulate_kernel<V><<<rows, kRowThreads, 0, stream>>>(                                         \
@@ -163,12 +264,86 @@ int ln_modulate(const void* x, int ldx, void* out, int ldo, int rows, int D, flo
     default: KR_LN_LAUNCH(8); break;
   }
 #undef KR_LN_LAUNCH
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) {
-    set_last_error("ln_modulate: launch failed: %s", cudaGetErrorString(e));
-    return KR_ERR_CUDA;
+  return launch_status("ln_modulate");
+}
+
+int ln_modulate_fp8(const void* x, int ldx, void* out, int ldo, int rows, int D, float eps,
+                    const void* w, const void* b, const void* mod, int mod_rows, int shift_idx,
+                    int scale_idx, int rows_per_frame, int row_offset, void* q, int ldq, float* scale_rows,
+                    cudaStream_t stream) {
+  const int rc = ln_check("ln_modulate_fp8", rows, D, ldx, out != nullptr ? ldo : 8, w, b, mod, rows_per_frame);
+  if (rc != KR_OK) return rc;
+  if (ldq % 8 != 0 || ldq < D) {
+    set_last_error("ln_modulate_fp8: unsupported ldq=%d for D=%d", ldq, D);
+    return KR_ERR_UNSUPPORTED_SHAPE;
   }
-  return KR_OK;
+  const int nv = (D / 8 + kRowThreads - 1) / kRowThreads;
+#define KR_LN_LAUNCH(V)                                                                            \
+  ln_modulate_fp8_kernel<V><<<rows, kRowThreads, 0, stream>>>(                                     \
+      static_cast<const uint16_t*>(x), ldx, static_cast<uint16_t*>(out), ldo, D, eps,              \
+      static_cast<const uint16_t*>(w), static_cast<const uint16_t*>(b),                            \
+      static_cast<const uint16_t*>(mod), mod_rows, shift_idx, scale_idx, rows_per_frame, row_offset, \
+      static_cast<uint8_t*>(q), ldq, scale_rows)
+  switch (nv) {
+    case 1: KR_LN_LAUNCH(1); break;
+    case 2: KR_LN_LAUNCH(2); break;
+    case 3: KR_LN_LAUNCH(3); break;
+    case 4: KR_LN_LAUNCH(4); break;
+    case 5: KR_LN_LAUNCH(5); break;
+    default: KR_LN_LAUNCH(8); break;
+  }
+#undef KR_LN_LAUNCH
+  return launch_status("ln_modulate_fp8");
+}
+
+// ---------------------------------------------------------------------------
+// Dynamic per-row e4m3 activation cast (torchao Float8DynamicActivation, PerRow): one CTA per row, the row in
+// registers, one read and one write; scale_rows[r] = amax_r / 448 is the row scale of the row-scaled FP8 GEMM.
+// Up to kRowThreads * 8 * kQuantMaxVec = 14336 channels (the FFN width of the 14B model is 13824).
+// ---------------------------------------------------------------------------
+static constexpr int kQuantMaxVec = 14;
+
+template <int kVec>
+__global__ void __launch_bounds__(kRowThreads)
+fp8_quantize_rows_kernel(const uint16_t* __restrict__ x, int ldx, int cols, uint8_t* __restrict__ q, int ldq,
+                         float* __restrict__ scale_rows) {
+  __shared__ float red[4];
+  const int row = blockIdx.x;
+  const uint16_t* xr = x + static_cast<size_t>(row) * ldx;
+  const int nvec = cols >> 3;
+  uint4 raw[kVec];
+#pragma unroll
+  for (int i = 0; i < kVec; ++i) {
+    const int vi = threadIdx.x + i * kRowThreads;
+    if (vi < nvec) raw[i] = *reinterpret_cast<const uint4*>(xr + vi * 8);
+  }
+  fp8_quantize_row<kVec>(raw, nvec, red, q + static_cast<size_t>(row) * ldq, scale_rows + row);
+}
+
+int fp8_quantize_rows(const void* x, int ldx, int rows, int cols, void* q, int ldq, float* scale_rows,
+                      cudaStream_t stream) {
+  if (cols <= 0 || cols % 8 != 0 || cols > kRowThreads * 8 * kQuantMaxVec || rows <= 0 || ldx % 8 != 0 ||
+      ldq % 8 != 0 || ldx < cols || ldq < cols) {
+    set_last_error("fp8_quantize_rows: unsupported rows=%d cols=%d ldx=%d ldq=%d", rows, cols, ldx, ldq);
+    return KR_ERR_UNSUPPORTED_SHAPE;
+  }
+  const int nv = (cols / 8 + kRowThreads - 1) / kRowThreads;
+#define KR_Q_LAUNCH(V)                                                                             \
+  fp8_quantize_rows_kernel<V><<<rows, kRowThreads, 0, stream>>>(                                   \
+      static_cast<const uint16_t*>(x), ldx, cols, static_cast<uint8_t*>(q), ldq, scale_rows)
+  switch (nv) {
+    case 1: KR_Q_LAUNCH(1); break;
+    case 2: KR_Q_LAUNCH(2); break;
+    case 3: KR_Q_LAUNCH(3); break;
+    case 4: KR_Q_LAUNCH(4); break;
+    case 5: KR_Q_LAUNCH(5); break;
+    case 6: KR_Q_LAUNCH(6); break;
+    case 7: case 8: KR_Q_LAUNCH(8); break;
+    case 9: case 10: KR_Q_LAUNCH(10); break;
+    default: KR_Q_LAUNCH(14); break;
+  }
+#undef KR_Q_LAUNCH
+  return launch_status("fp8_quantize_rows");
 }
 
 // ---------------------------------------------------------------------------

@@ -189,13 +189,19 @@ constexpr int kEpiScrPitch = 36;                       // floats per scratch row
 constexpr int kEpiScrFloats = 16 * kEpiScrPitch;       // one warp's 16 x 32 transpose buffer
 
 // The fragment of one warp (rows row0 .. row0+15 of the output, columns col_base + [0, BN)) -> fused epilogue.
-// Only the first n_valid columns (a multiple of 32) are stored; every accumulator is multiplied by `scale`.
-template <int BN, bool kBf16, int kEpi>
+// Only the first n_valid columns (a multiple of 32) are stored; every accumulator is multiplied by `scale`, or, with
+// kRowScale, by row_scale[row] and then by col_scale[col] (the row-scaled FP8 GEMM; rows >= M read no row scale).
+template <int BN, bool kBf16, int kEpi, bool kRowScale = false>
 KR_DEVICE void gemm_frag_epilogue(const float (&acc)[BN / 2], float* scr, int row0, int col_base, int n_valid,
-                                  float scale, const GemmParams& p) {
+                                  float scale, const GemmParams& p, const float* __restrict__ row_scale = nullptr,
+                                  const float* __restrict__ col_scale = nullptr) {
   const int lane = threadIdx.x & 31;
   const int row = row0 + (lane >> 1), half = lane & 1;
   const bool row_ok = row < p.M;
+  float sa = 0.f;
+  if constexpr (kRowScale) {
+    if (row_ok) sa = __ldg(row_scale + row);
+  }
   const uint16_t* gate_row = nullptr;
   if constexpr (kEpi == EPI_BIAS_GATE_RES) {
     const int g = row_ok ? (row + p.row_offset) / p.rows_per_gate : 0;
@@ -218,7 +224,13 @@ KR_DEVICE void gemm_frag_epilogue(const float (&acc)[BN / 2], float* scr, int ro
 #pragma unroll
         for (int q = 0; q < 4; ++q) {
           const float4 f = *reinterpret_cast<const float4*>(scr + (lane >> 1) * kEpiScrPitch + half * 16 + q * 4);
-          v[4 * q] = f.x * scale; v[4 * q + 1] = f.y * scale; v[4 * q + 2] = f.z * scale; v[4 * q + 3] = f.w * scale;
+          if constexpr (kRowScale) {
+            const float4 sw = __ldg(reinterpret_cast<const float4*>(col_scale + col_base + c * 32 + half * 16) + q);
+            v[4 * q] = f.x * sa * sw.x; v[4 * q + 1] = f.y * sa * sw.y;
+            v[4 * q + 2] = f.z * sa * sw.z; v[4 * q + 3] = f.w * sa * sw.w;
+          } else {
+            v[4 * q] = f.x * scale; v[4 * q + 1] = f.y * scale; v[4 * q + 2] = f.z * scale; v[4 * q + 3] = f.w * scale;
+          }
         }
         gemm_epilogue_row<kBf16, kEpi, 16>(v, row, col_base + c * 32 + half * 16, p, gate_row);
       }

@@ -1,6 +1,8 @@
-// kr_gemm_fp8.cu — FP8 (e4m3) wgmma GEMM with per-tensor scales + the dynamic activation quantisation kernels.
+// kr_gemm_fp8.cu — FP8 (e4m3) wgmma GEMM with per-tensor or per-row scales + the dynamic per-tensor activation
+// quantisation kernels (the per-row quantiser lives with the row kernels in kr_dit_elem.cu).
 //
-//   out[M,N] = epilogue( (Aq[M,K] @ Wq[N,K]^T) * scale_a * scale_w + bias[N] )      Aq, Wq e4m3, out bf16
+//   per tensor: out[M,N] = epilogue( (Aq[M,K] @ Wq[N,K]^T) * scale_a * scale_w + bias[N] )    Aq, Wq e4m3, out bf16
+//   per row   : out[M,N] = epilogue( (Aq[M,K] @ Wq[N,K]^T) * scale_a[m] * scale_w[n] + bias[N] )
 //
 // Replaces, on the reference path, what `quantize_(transformer, Float8DynamicActivationFloat8WeightConfig(
 // granularity=PerTensor()))` (release_server.py:179-182, `enable_fp8: true`) turns every nn.Linear into: torchao's
@@ -8,6 +10,9 @@
 // followed by torch._scaled_mm (cuBLASLt FP8, fp32 accumulation, bf16 output) — here a hand-written
 // wgmma e4m3 kernel with the same fused epilogues as the bf16 GEMM (bias, GELU, gate + residual, ...).
 // torchao is absent from the image: the algorithm is restated from its published definition (oracle/fp8_oracle.py).
+// granularity=PerRow() gives one scale per activation row and one per weight output channel: the same kernel, with
+// the two scale vectors applied in the epilogue (torch._scaled_mm with scale_a [M, 1], scale_b [1, N]);
+// oracle/fp8_rowwise_oracle.py restates it.
 //
 // Kernel structure = kr_gemm.cu (persistent 1 CTA/SM, two consumer warpgroups with register accumulators, a TMA
 // warpgroup), with byte-sized elements: a 128-byte swizzle row holds 128 k-elements, one wgmma consumes K = 32
@@ -29,10 +34,14 @@ constexpr int F8_SCR_BYTES = 8 * kEpiScrFloats * 4;
 constexpr int F8_SMEM = F8_STAGES * F8_STAGE_BYTES + F8_SCR_BYTES + 1024 + 256;
 }  // namespace
 
-template <int kEpi>
+// per tensor: scale_a -> one fp32 in device memory, scale_w a float; per row: scale_a -> [M], scale_w -> [N] fp32
+template <bool kRowwise> struct Fp8ScaleW { using type = float; };
+template <> struct Fp8ScaleW<true> { using type = const float*; };
+
+template <int kEpi, bool kRowwise>
 __global__ void __launch_bounds__(F8_THREADS, 1)
 gemm_fp8_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
-                const GemmParams p, const float* __restrict__ scale_a, const float scale_w) {
+                const GemmParams p, const float* __restrict__ scale_a, const typename Fp8ScaleW<kRowwise>::type scale_w) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
                                              ~static_cast<uintptr_t>(1023));
@@ -83,7 +92,8 @@ gemm_fp8_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constan
   const int wg = warp >> 2;
   const uint32_t a_base = smem_u32(smem_a) + wg * 64 * F8_BK, b_base = smem_u32(smem_b);
   float* scr = scratch + warp * kEpiScrFloats;
-  const float s = __ldg(scale_a) * scale_w;       // dequantisation: per-tensor activation x weight scale
+  float s = 1.f;
+  if constexpr (!kRowwise) s = __ldg(scale_a) * scale_w;   // dequantisation: per-tensor activation x weight scale
   int stage = 0;
   uint32_t phase = 0;
   for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
@@ -91,8 +101,12 @@ gemm_fp8_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constan
     float acc[F8_BN / 2];
     gemm_mainloop<F8_BN, 2>(acc, a_base, b_base, F8_A_BYTES, F8_B_BYTES, F8_STAGES, full_bar, empty_bar, stage, phase,
                             0, num_k);
-    gemm_frag_epilogue<F8_BN, true, kEpi>(acc, scr, m_blk * F8_BM + wg * 64 + (warp & 3) * 16, n_blk * F8_BN, F8_BN,
-                                          s, p);
+    if constexpr (kRowwise)
+      gemm_frag_epilogue<F8_BN, true, kEpi, true>(acc, scr, m_blk * F8_BM + wg * 64 + (warp & 3) * 16, n_blk * F8_BN,
+                                                  F8_BN, s, p, scale_a, scale_w);
+    else
+      gemm_frag_epilogue<F8_BN, true, kEpi>(acc, scr, m_blk * F8_BM + wg * 64 + (warp & 3) * 16, n_blk * F8_BN, F8_BN,
+                                            s, p);
   }
 }
 
@@ -173,9 +187,9 @@ int fp8_quantize(const void* x, long ld, int rows, int cols, void* q, long ldq, 
 // ---------------------------------------------------------------------------
 // host launcher
 // ---------------------------------------------------------------------------
-template <int kEpi>
+template <int kEpi, bool kRowwise>
 static int launch_fp8(const void* a, int lda, const void* w, int ldw, const GemmParams& p, const float* scale_a,
-                      float scale_w, cudaStream_t stream) {
+                      typename Fp8ScaleW<kRowwise>::type scale_w, cudaStream_t stream) {
   CUtensorMap ta, tb;
   // byte tensors: [rows, K] uint8, box [128 | 256 rows, 128 bytes], SWIZZLE_128B
   const uint64_t da[2] = {static_cast<uint64_t>(p.K), static_cast<uint64_t>(p.M)};
@@ -188,7 +202,7 @@ static int launch_fp8(const void* a, int lda, const void* w, int ldw, const Gemm
   const uint32_t bb[2] = {F8_BK, F8_BN};
   rc = make_tmap_u8(&tb, w, 2, db, sb, bb, 128);
   if (rc != KR_OK) return rc;
-  auto kern = gemm_fp8_kernel<kEpi>;
+  auto kern = gemm_fp8_kernel<kEpi, kRowwise>;
   static bool attr_set = false;
   if (!attr_set) {
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, F8_SMEM);
@@ -210,27 +224,54 @@ static int launch_fp8(const void* a, int lda, const void* w, int ldw, const Gemm
   return KR_OK;
 }
 
-int gemm_fp8_tn(int epi, const void* a, int lda, const void* w, int ldw, const GemmParams& p, const float* scale_a,
-                float scale_w, cudaStream_t stream) {
+static int check_fp8(const char* who, int epi, int lda, int ldw, const GemmParams& p) {
   if (p.M <= 0 || p.N <= 0 || p.K <= 0 || p.N % F8_BN != 0 || p.K % 16 != 0 || lda % 16 != 0 || ldw % 16 != 0 ||
       p.ldc % 8 != 0) {
-    set_last_error("gemm_fp8: unsupported shape M=%d N=%d K=%d (need N %% 128 == 0, K / ld %% 16 == 0)", p.M, p.N, p.K);
+    set_last_error("%s: unsupported shape M=%d N=%d K=%d (need N %% 128 == 0, K / ld %% 16 == 0)", who, p.M, p.N, p.K);
     return KR_ERR_UNSUPPORTED_SHAPE;
   }
   if ((epi == EPI_BIAS_GATE_RES || epi == EPI_BIAS_RES || epi == EPI_MUL) && p.residual == nullptr) {
-    set_last_error("gemm_fp8: residual epilogue without residual pointer");
+    set_last_error("%s: residual epilogue without residual pointer", who);
     return KR_ERR_INVALID_ARG;
   }
+  return KR_OK;
+}
+
+int gemm_fp8_tn(int epi, const void* a, int lda, const void* w, int ldw, const GemmParams& p, const float* scale_a,
+                float scale_w, cudaStream_t stream) {
+  const int rc = check_fp8("gemm_fp8", epi, lda, ldw, p);
+  if (rc != KR_OK) return rc;
   if (scale_a == nullptr) {
     set_last_error("gemm_fp8: null activation scale");
     return KR_ERR_INVALID_ARG;
   }
   switch (epi) {
-    case EPI_BIAS: return launch_fp8<EPI_BIAS>(a, lda, w, ldw, p, scale_a, scale_w, stream);
-    case EPI_BIAS_GELU: return launch_fp8<EPI_BIAS_GELU>(a, lda, w, ldw, p, scale_a, scale_w, stream);
-    case EPI_BIAS_GATE_RES: return launch_fp8<EPI_BIAS_GATE_RES>(a, lda, w, ldw, p, scale_a, scale_w, stream);
-    case EPI_BIAS_RES: return launch_fp8<EPI_BIAS_RES>(a, lda, w, ldw, p, scale_a, scale_w, stream);
+    case EPI_BIAS: return launch_fp8<EPI_BIAS, false>(a, lda, w, ldw, p, scale_a, scale_w, stream);
+    case EPI_BIAS_GELU: return launch_fp8<EPI_BIAS_GELU, false>(a, lda, w, ldw, p, scale_a, scale_w, stream);
+    case EPI_BIAS_GATE_RES: return launch_fp8<EPI_BIAS_GATE_RES, false>(a, lda, w, ldw, p, scale_a, scale_w, stream);
+    case EPI_BIAS_RES: return launch_fp8<EPI_BIAS_RES, false>(a, lda, w, ldw, p, scale_a, scale_w, stream);
     default: set_last_error("gemm_fp8: unsupported epilogue %d", epi); return KR_ERR_INVALID_ARG;
+  }
+}
+
+int gemm_fp8_rowwise_tn(int epi, const void* a, int lda, const void* w, int ldw, const GemmParams& p,
+                        const float* scale_a, const float* scale_w, cudaStream_t stream) {
+  const int rc = check_fp8("gemm_fp8_rowwise", epi, lda, ldw, p);
+  if (rc != KR_OK) return rc;
+  if (scale_a == nullptr || scale_w == nullptr) {
+    set_last_error("gemm_fp8_rowwise: null row or channel scales");
+    return KR_ERR_INVALID_ARG;
+  }
+  if (reinterpret_cast<uintptr_t>(scale_w) % 16 != 0) {
+    set_last_error("gemm_fp8_rowwise: channel scales must be 16-byte aligned");
+    return KR_ERR_INVALID_ARG;
+  }
+  switch (epi) {
+    case EPI_BIAS: return launch_fp8<EPI_BIAS, true>(a, lda, w, ldw, p, scale_a, scale_w, stream);
+    case EPI_BIAS_GELU: return launch_fp8<EPI_BIAS_GELU, true>(a, lda, w, ldw, p, scale_a, scale_w, stream);
+    case EPI_BIAS_GATE_RES: return launch_fp8<EPI_BIAS_GATE_RES, true>(a, lda, w, ldw, p, scale_a, scale_w, stream);
+    case EPI_BIAS_RES: return launch_fp8<EPI_BIAS_RES, true>(a, lda, w, ldw, p, scale_a, scale_w, stream);
+    default: set_last_error("gemm_fp8_rowwise: unsupported epilogue %d", epi); return KR_ERR_INVALID_ARG;
   }
 }
 

@@ -47,6 +47,19 @@ bool gemm_sk_preferred(int epi, int M, int N, int K);
 int fp8_quantize(const void* x, long ld, int rows, int cols, void* q, long ldq, float* state, cudaStream_t stream);
 int gemm_fp8_tn(int epi, const void* a, int lda, const void* w, int ldw, const GemmParams& p, const float* scale_a,
                 float scale_w, cudaStream_t stream);
+// Row-scaled FP8 (torchao PerRow): per-row e4m3 cast (kr_dit_elem.cu), LayerNorm with e4m3 output (kr_dit_elem.cu)
+// and the FP8 GEMM with [M] row and [N] channel scales (kr_gemm_fp8.cu).  Declared weak: the launch-recording build
+// of the API layer (tests/test_block_fwd_cpu.py) links no kernel files and must still export the kr_* entry points;
+// there they report KR_ERR_CUDA, in the library they are always defined.
+__attribute__((weak)) int fp8_quantize_rows(const void* x, int ldx, int rows, int cols, void* q, int ldq,
+                                            float* scale_rows, cudaStream_t stream);
+__attribute__((weak)) int ln_modulate_fp8(const void* x, int ldx, void* out, int ldo, int rows, int D, float eps,
+                                          const void* w, const void* b, const void* mod, int mod_rows, int shift_idx,
+                                          int scale_idx, int rows_per_frame, int row_offset, void* q, int ldq,
+                                          float* scale_rows, cudaStream_t stream);
+__attribute__((weak)) int gemm_fp8_rowwise_tn(int epi, const void* a, int lda, const void* w, int ldw,
+                                              const GemmParams& p, const float* scale_a, const float* scale_w,
+                                              cudaStream_t stream);
 // 2-CTA cluster variant (W multicast to both CTAs, 128x256 tile per CTA), kr_gemm2.cu; N % 256 == 0
 int gemm2_tn(int dtype, int epi, const void* a, int lda, const void* w, int ldw, const GemmParams& p,
              cudaStream_t stream);

@@ -26,16 +26,24 @@ from typing import Dict, List, Optional
 import torch
 import torch.nn as nn
 
-from . import ops
+from . import fp8, ops
 
 
-def _linear(x: torch.Tensor, lin: nn.Linear, **kw) -> torch.Tensor:
-    """nn.Linear of a DiT block on the GEMM kernels: bf16 by default, FP8 (dynamic per-tensor activation cast +
-    e4m3 wgmma GEMM) when ``realtime_video_b200.fp8.quantize_`` attached quantised weights to the module."""
+def _linear(x, lin: nn.Linear, **kw) -> torch.Tensor:
+    """nn.Linear of a DiT block on the GEMM kernels: bf16 by default, FP8 (dynamic activation cast + e4m3 wgmma GEMM)
+    when ``realtime_video_b200.fp8.quantize_`` attached quantised weights to the module, with the granularity it
+    attached: per tensor, or per row (``x`` may then be an ``ops.Fp8Rows`` the LayerNorm already cast)."""
     q = getattr(lin, "_kr_fp8", None)
     if q is None:
         return ops.gemm(x, lin.weight, lin.bias, **kw)
+    if fp8.is_rowwise(lin):
+        return ops.linear_fp8_rowwise(x, q[0], q[1], lin.bias, **kw)
     return ops.linear_fp8(x, q[0], q[1], lin.bias, **kw)
+
+
+def _rowwise(*lins: nn.Module) -> bool:
+    """Every one of ``lins`` runs the PerRow FP8 GEMM: their common input can be cast to e4m3 once, by its producer."""
+    return all(fp8.is_rowwise(m) for m in lins)
 
 
 def rope_angles(max_seq_len: int, dim: int, theta: float = 10000.0) -> torch.Tensor:
@@ -398,6 +406,8 @@ class CausalWanModel(nn.Module):
         if cache is not None and cache["is_init"]:
             k, v = cache["k"], cache["v"]
         else:
+            if _rowwise(ca.k, ca.v):
+                ctx = ops.fp8_quantize_rows(ctx)        # one per-row cast of the prompt feeds both projections
             k = _linear(ctx, ca.k)
             ops.rmsnorm(k, ca.norm_k.weight, ca.eps, out=k)
             v = _linear(ctx, ca.v)
@@ -458,22 +468,34 @@ class CausalWanModel(nn.Module):
             return self._block_one_call(blk, x, e0, grid, kv_cache, crossattn_cache, current_start, mask)
         r0 = 0 if self.sp is None else self.sp.rank * x.shape[0]       # global index of my first row
         emod = ops.add_modulation(blk.modulation, e0)                    # [F, 6, D]
-        h = ops.ln_modulate(x, eps=blk.eps, mod=emod, shift_idx=0, scale_idx=1, rows_per_frame=fs,
-                            row_offset=r0)
+        sa, ca = blk.self_attn, blk.cross_attn
+        # PerRow FP8: a LayerNorm whose every consumer is a row-scaled FP8 linear writes e4m3 bytes + row scales
+        # instead of its bf16 output (ln_modulate_fp8); `buf` is the bf16 scratch row buffer while there is one
+        if _rowwise(*((sa.to_qkv,) if sa.fused_projections else (sa.q, sa.k, sa.v))):
+            h = ops.ln_modulate_fp8(x, eps=blk.eps, mod=emod, shift_idx=0, scale_idx=1, rows_per_frame=fs,
+                                    row_offset=r0)
+            buf = None
+        else:
+            h = buf = ops.ln_modulate(x, eps=blk.eps, mod=emod, shift_idx=0, scale_idx=1, rows_per_frame=fs,
+                                      row_offset=r0)
         y = self._self_attention(blk, h, grid, kv_cache, current_start, mask)
-        sa = blk.self_attn
         _linear(y, sa.o, epilogue=ops.EPI_BIAS_GATE_RES, residual=x,
                  gate=emod[:, 2], rows_per_gate=fs, out=x, row_offset=r0)
         n3 = blk.norm3
-        if isinstance(n3, nn.LayerNorm):
-            hc = ops.ln_modulate(x, eps=n3.eps, weight=n3.weight, bias=n3.bias, out=h)
+        if isinstance(n3, nn.LayerNorm) and _rowwise(ca.q):
+            hc = ops.ln_modulate_fp8(x, eps=n3.eps, weight=n3.weight, bias=n3.bias)
+        elif isinstance(n3, nn.LayerNorm):
+            hc = buf = ops.ln_modulate(x, eps=n3.eps, weight=n3.weight, bias=n3.bias, out=buf)
         else:
-            hc = x          # cross_attn_norm=False: the residual stream itself; `h` stays the scratch buffer
+            hc = x          # cross_attn_norm=False: the residual stream itself; `buf` stays the scratch buffer
         y = self._cross_attention(blk, hc, ctx, crossattn_cache)
-        ca = blk.cross_attn
         _linear(y, ca.o, epilogue=ops.EPI_BIAS_RES, residual=x, out=x)
-        h = ops.ln_modulate(x, eps=blk.eps, mod=emod, shift_idx=3, scale_idx=4, rows_per_frame=fs, out=h,
-                            row_offset=r0)
+        if _rowwise(blk.ffn[0]):
+            h = ops.ln_modulate_fp8(x, eps=blk.eps, mod=emod, shift_idx=3, scale_idx=4, rows_per_frame=fs,
+                                    row_offset=r0)
+        else:
+            h = ops.ln_modulate(x, eps=blk.eps, mod=emod, shift_idx=3, scale_idx=4, rows_per_frame=fs, out=buf,
+                                row_offset=r0)
         hid = _linear(h, blk.ffn[0], epilogue=ops.EPI_BIAS_GELU)
         _linear(hid, blk.ffn[2], epilogue=ops.EPI_BIAS_GATE_RES, residual=x,
                  gate=emod[:, 5], rows_per_gate=fs, out=x, row_offset=r0)

@@ -13,7 +13,8 @@ resolving to the reference checkout, independent of the ``sys.path`` order:
     demo_utils.vae             -> realtime_video_b200.vae           (VAEDecoderWrapperSingle, ZERO_VAE_CACHE, ...; demo_utils/vae.py:150-195)
     wan.modules.causal_model   -> realtime_video_b200.dit           (CausalWanModel; wan/modules/causal_model.py:526)
     torchao.quantization.quant_api -> realtime_video_b200.fp8       (quantize_, Float8DynamicActivationFloat8WeightConfig,
-                                                                     PerTensor: the `enable_fp8` lines release_server.py:179-182)
+                                                                     PerTensor: the `enable_fp8` lines release_server.py:179-182;
+                                                                     PerRow: the same lines with granularity=PerRow() also resolve)
 
 The served module IS the product module (same object under both names), so ``isinstance`` checks and class
 identity hold across the two spellings.  The reference's ``CausalInferencePipeline`` and ``GenerationSession``
@@ -39,6 +40,7 @@ ALIASES = {
     "demo_utils.vae": "realtime_video_b200.vae",
     "wan.modules.causal_model": "realtime_video_b200.dit",
     # `enable_fp8: true` (release_server.py:179-182): quantize_ / Float8DynamicActivationFloat8WeightConfig / PerTensor
+    # (or PerRow)
     "torchao.quantization.quant_api": "realtime_video_b200.fp8",
 }
 

@@ -11,6 +11,11 @@ block schedule (realtime_video_b200/dit.py ``_linear``) then runs ``kr_fp8_quant
 bf16.  ``realtime_video_b200.dropin`` serves this module as ``torchao.quantization.quant_api`` so the server's own three
 lines above work unchanged.
 
+``granularity=PerRow()`` (or ``[PerRow(), PerRow()]``) is torchao's row-wise variant: one scale per activation row
+(token) and one per weight output channel, so one outlier sets the scale of its own row only, and the scales do not
+depend on how the rows are split across GPUs.  The block schedule then runs ``kr_gemm_fp8_rowwise`` fed by
+``kr_ln_modulate_fp8`` (the LayerNorm writes e4m3 bytes and row scales directly) or ``kr_fp8_quantize_rows``.
+
 Numerics are a separate tier from the bf16 headline: e4m3 has 3 mantissa bits; tests state the tolerance against the
 fp8 oracle (same quantisation, fp32 matmul) and against the bf16 path.
 """
@@ -26,11 +31,25 @@ class PerTensor:
     """Granularity marker (torchao.quantization.PerTensor)."""
 
 
+class PerRow:
+    """Granularity marker (torchao.quantization.PerRow): per-row activation scales, per-output-channel weight scales."""
+
+
 class Float8DynamicActivationFloat8WeightConfig:
+    """``granularity``: ``PerTensor()`` or ``PerRow()``, alone or as an (activation, weight) pair of the same kind."""
+
     def __init__(self, granularity=None, **unused):
-        if granularity is not None and not isinstance(granularity, PerTensor):
-            raise NotImplementedError("only the per-tensor granularity the reference server uses is implemented")
-        self.granularity = granularity or PerTensor()
+        g = PerTensor() if granularity is None else granularity
+        if isinstance(g, (list, tuple)):
+            if len(g) != 2:
+                raise ValueError(f"granularity pair must have two entries, got {len(g)}")
+            if type(g[0]) is not type(g[1]):
+                raise ValueError("activation and weight granularity must be of the same kind, got "
+                                 f"{type(g[0]).__name__} and {type(g[1]).__name__}")
+            g = g[0]
+        if not isinstance(g, (PerTensor, PerRow)):
+            raise NotImplementedError(f"granularity {type(g).__name__} is not implemented (PerTensor or PerRow)")
+        self.granularity = g
 
 
 @torch.no_grad()
@@ -42,12 +61,30 @@ def quantize_weight(w: torch.Tensor):
 
 
 @torch.no_grad()
+def quantize_weight_rows(w: torch.Tensor):
+    """w [N, K] -> (e4m3 bytes as uint8 [N, K], fp32 [N] dequantisation scales amax_n / 448), one per output
+    channel: w_q[n] = sat(w[n] * 448 / amax_n)."""
+    amax = w.detach().float().abs().amax(dim=1, keepdim=True).clamp(min=1e-12)
+    mul = torch.full_like(amax, E4M3_MAX) / amax          # a true division, as in the kernels
+    q = (w.detach().float() * mul).clamp(-E4M3_MAX, E4M3_MAX).to(torch.float8_e4m3fn)
+    return q.view(torch.uint8).contiguous(), (amax / E4M3_MAX).squeeze(1).contiguous()
+
+
+def is_rowwise(lin: nn.Module) -> bool:
+    """True when :func:`quantize_` attached per-row (PerRow) FP8 weights to ``lin``."""
+    return isinstance(getattr(lin, "_kr_fp8_granularity", None), PerRow)
+
+
+@torch.no_grad()
 def quantize_(module: nn.Module, config=None, filter_fn=None) -> nn.Module:
     """In-place, like torchao's: every ``nn.Linear`` inside the DiT blocks of ``module`` (a WanDiffusionWrapper, a
     CausalWanModel or any container of CausalWanAttentionBlock) gets FP8 weights.  The bf16 weights stay in place
-    (state_dict unchanged); call ``dequantize_`` to go back."""
+    (state_dict unchanged); call ``dequantize_`` to go back.  PerTensor attaches ``(w_q, scale_w float)``, PerRow
+    ``(w_q, scale_w fp32 [N])`` on the weight's device."""
     if config is not None and not isinstance(config, Float8DynamicActivationFloat8WeightConfig):
         raise NotImplementedError(f"unsupported quantisation config {type(config).__name__}")
+    gran = config.granularity if config is not None else PerTensor()
+    quant = quantize_weight_rows if isinstance(gran, PerRow) else quantize_weight
     from .dit import CausalWanAttentionBlock
     n = 0
     for blk in module.modules():
@@ -56,7 +93,8 @@ def quantize_(module: nn.Module, config=None, filter_fn=None) -> nn.Module:
         for name, lin in blk.named_modules():
             if isinstance(lin, nn.Linear) and lin.weight.shape[0] % 256 == 0 and lin.weight.shape[1] % 16 == 0 and \
                     (filter_fn is None or filter_fn(lin, name)):
-                lin._kr_fp8 = quantize_weight(lin.weight)
+                lin._kr_fp8 = quant(lin.weight)
+                lin._kr_fp8_granularity = gran
                 n += 1
     if n == 0:
         raise ValueError("quantize_: no DiT block linears found in the module")
@@ -67,4 +105,6 @@ def dequantize_(module: nn.Module) -> nn.Module:
     for lin in module.modules():
         if isinstance(lin, nn.Linear) and hasattr(lin, "_kr_fp8"):
             del lin._kr_fp8
+            if hasattr(lin, "_kr_fp8_granularity"):
+                del lin._kr_fp8_granularity
     return module
