@@ -304,5 +304,8 @@ int kr_rgb8_to_jpeg(const unsigned char* rgb, int frames, int height, int width,
 /* The quantised attention tier (kr_sage_quantize / kr_sage_attn) is declared in its own header: its entry points and
  * kernels are one translation unit, kr_sage.cu, outside the API layer above. */
 #include "krea_b200_sage.h"
+/* The FP8 tier of the VAE decoder's convolutions (kr_vae_conv_fp8 / kr_vae_rmsnorm_silu_fp8): likewise its own header;
+ * the entry points live with the kernels in kr_vae.cu. */
+#include "krea_b200_vae_fp8.h"
 
 #endif /* KREA_B200_H_ */

@@ -165,6 +165,13 @@ SAGE_SIGNATURES = {
     "kr_sage_attn": [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _f, _vp],
 }
 
+# the FP8 tier of the VAE decoder's convolutions (include/krea_b200_vae_fp8.h, kr_vae.cu); every function returns int
+VAE_FP8_SIGNATURES = {
+    "kr_vae_conv_fp8": [_i, _i, _i, _vp, _i, _vp, _vp, _f, _i, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _vp, _l, _l,
+                        _vp, _l, _l, _f, _vp, _vp, _l, _l, _vp, _vp],
+    "kr_vae_rmsnorm_silu_fp8": [_vp, _vp, _vp, _l, _i, _f, _vp],
+}
+
 
 def load() -> ctypes.CDLL:
     """Load the shared library (building is the caller's job: ``__graft_entry__.build``)."""
@@ -191,7 +198,7 @@ def load() -> ctypes.CDLL:
         if hasattr(lib, "kr_jpeg_workspace_bytes"):
             lib.kr_jpeg_workspace_bytes.restype = _sz
             lib.kr_jpeg_workspace_bytes.argtypes = [_i, _i, _i]
-        for name, argtypes in {**SIGNATURES, **SAGE_SIGNATURES}.items():
+        for name, argtypes in {**SIGNATURES, **SAGE_SIGNATURES, **VAE_FP8_SIGNATURES}.items():
             fn = getattr(lib, name, None)
             if fn is None:
                 continue   # checked by tests/test_abi.py against the header

@@ -18,9 +18,13 @@
 //   (vae.py:39-54, :184-186) for the NEXT conv's input, or clamp -> fp32 NCHW pixels.
 // Small HBM-bound kernels: latent un-scaling + conv2 (vae_block3.py:205-214), RMS_norm+SiLU,
 //   nearest 2x upsample (vae.py:57-63), row softmax for the middle attention block.
+#include "../../include/krea_b200.h"
 #include "kr_common.cuh"
 #include "kr_ops.h"
 
+#include <cuda_fp8.h>
+
+#include <cmath>
 #include <cstdlib>
 
 namespace kr {
@@ -68,12 +72,15 @@ KR_DEVICE float load16(const uint16_t* p) {
 // warp's 16; channel pairs 8*nb + 2*(lane%4)): bias, optional residual, rounding, raw store, fused
 // RMS_norm*sqrt(C)*gamma -> SiLU store (the sum of squares is reduced over the quad), or clamp -> fp32 NCHW
 // pixels (N == 16 head).
-template <int N, bool kBf16>
-KR_DEVICE void conv_epilogue_frag(const ConvParams& p, float (&acc)[N / 2], int t, const int (&hh)[2],
-                                  const int (&ww)[2], int lane) {
+// kNormF8: out_norm holds e4m3 bytes e4m3(v * p.norm_q_scale) of the 16-bit value v (the FP8 tier's conv inputs).
+// kSplit == 2: the fragment holds channels [c0, c0 + N/2) of the pixel and the other consumer warpgroup holds the rest;
+// the sum of squares of the norm is completed through `red` (128 floats of shared memory) and named barrier 1.
+template <int N, bool kBf16, bool kNormF8 = false, int kSplit = 1>
+KR_DEVICE void conv_epilogue_frag(const ConvParams& p, float (&acc)[N / 2 / kSplit], int t, const int (&hh)[2],
+                                  const int (&ww)[2], int lane, int c0 = 0, float* red = nullptr) {
   const uint16_t* bias = reinterpret_cast<const uint16_t*>(p.bias);
   const uint16_t* gamma = reinterpret_cast<const uint16_t*>(p.gamma);
-  const int cq = 2 * (lane & 3);
+  const int cq = c0 + 2 * (lane & 3);
 #pragma unroll
   for (int r = 0; r < 2; ++r) {
     const int h = hh[r], w = ww[r];
@@ -105,7 +112,7 @@ KR_DEVICE void conv_epilogue_frag(const ConvParams& p, float (&acc)[N / 2], int 
       float sumsq = 0.f;
       // ---- pass 1: bias (+ residual), round, raw store, sum of squares ----
 #pragma unroll
-      for (int nb = 0; nb < N / 8; ++nb) {
+      for (int nb = 0; nb < N / 8 / kSplit; ++nb) {
         const int c = nb * 8 + cq;
         float f0 = acc[4 * nb + 2 * r], f1 = acc[4 * nb + 2 * r + 1];
         if (bias != nullptr) {
@@ -130,20 +137,36 @@ KR_DEVICE void conv_epilogue_frag(const ConvParams& p, float (&acc)[N / 2], int 
       if (p.out_norm != nullptr) {
         sumsq += __shfl_xor_sync(0xffffffffu, sumsq, 1);
         sumsq += __shfl_xor_sync(0xffffffffu, sumsq, 2);
+        if constexpr (kSplit == 2) {
+          // pixel row of the warpgroup's m64 fragment; both halves add the two partial sums in the same order
+          const int prow = ((threadIdx.x >> 5) & 3) * 16 + (lane >> 2) + 8 * r;
+          if ((lane & 3) == 0) red[(threadIdx.x >> 7) * 64 + prow] = sumsq;
+          named_bar_sync(1, 256);
+          sumsq = red[prow] + red[64 + prow];
+          named_bar_sync(1, 256);
+        }
         const float nrm = rnd16<kBf16>(sqrtf(sumsq));
         const float inv = 1.0f / fmaxf(nrm, 1e-30f);
         if (ok) {
           uint16_t* onrm = reinterpret_cast<uint16_t*>(p.out_norm) + t * p.norm_frame + pix * p.norm_pix;
+          uint8_t* onrm8 = reinterpret_cast<uint8_t*>(p.out_norm) + t * p.norm_frame + pix * p.norm_pix;
 #pragma unroll
-          for (int nb = 0; nb < N / 8; ++nb) {
+          for (int nb = 0; nb < N / 8 / kSplit; ++nb) {
             const int c = nb * 8 + cq;
             const float2 g = unpack16<kBf16>(__ldg(reinterpret_cast<const unsigned int*>(gamma + c)));
             float a = rnd16<kBf16>(acc[4 * nb + 2 * r] * inv);
             float b = rnd16<kBf16>(acc[4 * nb + 2 * r + 1] * inv);
             a = rnd16<kBf16>(rnd16<kBf16>(a * p.norm_scale) * g.x);
             b = rnd16<kBf16>(rnd16<kBf16>(b * p.norm_scale) * g.y);
-            *reinterpret_cast<uint32_t*>(onrm + c) =
-                pack16<kBf16>(a / (1.0f + __expf(-a)), b / (1.0f + __expf(-b)));
+            if constexpr (kNormF8) {
+              const float qa = rnd16<kBf16>(a / (1.0f + __expf(-a))) * p.norm_q_scale;
+              const float qb = rnd16<kBf16>(b / (1.0f + __expf(-b))) * p.norm_q_scale;
+              *reinterpret_cast<__nv_fp8x2_storage_t*>(onrm8 + c) =
+                  __nv_cvt_float2_to_fp8x2(make_float2(qa, qb), __NV_SATFINITE, __NV_E4M3);
+            } else {
+              *reinterpret_cast<uint32_t*>(onrm + c) =
+                  pack16<kBf16>(a / (1.0f + __expf(-a)), b / (1.0f + __expf(-b)));
+            }
           }
         }
       }
@@ -151,7 +174,7 @@ KR_DEVICE void conv_epilogue_frag(const ConvParams& p, float (&acc)[N / 2], int 
   }
 }
 
-template <int CIN, int N, bool kBf16>
+template <int CIN, int N, bool kBf16, bool kNormF8 = false>
 __global__ void __launch_bounds__(kConvThreads, 1)
 conv_igemm_kernel(const __grid_constant__ CUtensorMap tm_in64, const __grid_constant__ CUtensorMap tm_in32,
                   const __grid_constant__ CUtensorMap tm_w64, const __grid_constant__ CUtensorMap tm_w32,
@@ -289,7 +312,7 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tm_in64, const __grid_cons
       hh[r] = (rem / tiles_w) * p.TH + px / p.TW;
       ww[r] = (rem % tiles_w) * p.TW + px % p.TW;
     }
-    conv_epilogue_frag<N, kBf16>(p, acc, t, hh, ww, lane);
+    conv_epilogue_frag<N, kBf16, kNormF8>(p, acc, t, hh, ww, lane);
   }
 }
 
@@ -326,7 +349,7 @@ struct HaloCfg {
 static constexpr int kHaloThreads = 384;
 
 
-template <int CIN, int N, bool kBf16>
+template <int CIN, int N, bool kBf16, bool kNormF8 = false>
 __global__ void __launch_bounds__(kHaloThreads, 1)
 conv_halo_kernel(const __grid_constant__ CUtensorMap tm_in, const __grid_constant__ CUtensorMap tm_w,
                  const ConvParams p) {
@@ -462,12 +485,12 @@ conv_halo_kernel(const __grid_constant__ CUtensorMap tm_in, const __grid_constan
         hh[r] = (rem / items_w) * 16 + (px >> 3);
         ww[r] = (rem % items_w) * 16 + u * 8 + (px & 7);
       }
-      conv_epilogue_frag<N, kBf16>(p, acc[mh], t, hh, ww, lane);
+      conv_epilogue_frag<N, kBf16, kNormF8>(p, acc[mh], t, hh, ww, lane);
     }
   }
 }
 
-template <int CIN, int N, bool kBf16>
+template <int CIN, int N, bool kBf16, bool kNormF8 = false>
 static int launch_conv_halo(const void* in, int t_in, const void* wgt, int w_rows, const ConvParams& p,
                             cudaStream_t stream) {
   using Cfg = HaloCfg<CIN, N>;
@@ -485,7 +508,7 @@ static int launch_conv_halo(const void* in, int t_in, const void* wgt, int w_row
   const uint32_t wbox[2] = {64, static_cast<uint32_t>(N)};
   rc = make_tmap_nd(&tw, wgt, 2, wdims, wstr, wbox, kBf16, 128);
   if (rc != KR_OK) return rc;
-  auto kern = conv_halo_kernel<CIN, N, kBf16>;
+  auto kern = conv_halo_kernel<CIN, N, kBf16, kNormF8>;
   static bool attr_set = false;
   if (!attr_set) {
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes);
@@ -510,7 +533,7 @@ static int launch_conv_halo(const void* in, int t_in, const void* wgt, int w_row
 // ---------------------------------------------------------------------------
 // host launcher
 // ---------------------------------------------------------------------------
-template <int CIN, int N, bool kBf16>
+template <int CIN, int N, bool kBf16, bool kNormF8 = false>
 static int launch_conv(const void* in, int t_in, const void* wgt, int w_rows, const ConvParams& p,
                        cudaStream_t stream) {
   using Cfg = ConvCfg<CIN, N>;
@@ -538,7 +561,7 @@ static int launch_conv(const void* in, int t_in, const void* wgt, int w_rows, co
     rc = make_tmap_nd(&w32, wgt, 2, wdims, wstr, wbox32, kBf16, 64);
     if (rc != KR_OK) return rc;
   }
-  auto kern = conv_igemm_kernel<CIN, N, kBf16>;
+  auto kern = conv_igemm_kernel<CIN, N, kBf16, kNormF8>;
   static bool attr_set = false;
   if (!attr_set) {
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize,
@@ -616,14 +639,434 @@ int vae_conv(int dtype, int cin, int n, const void* in, int t_in, const void* wg
                     : dispatch_conv<false>(cin, n, in, t_in, wgt, w_rows, p, stream);
 }
 
+// =============================================================================================
+// FP8 (e4m3) tier of the convolutions whose input is a normalised tensor (residual.2 / residual.6 of every
+// ResidualBlock and head.2).  The input holds e4m3(v * s) of the 16-bit SiLU(RMS_norm(x) * sqrt(C) * gamma) value v,
+// written by the producer's epilogue, with the static scale s = 448 / (sqrt(C) * max|gamma|): |v| <= sqrt(C) max|gamma|
+// (a unit vector's entries are <= 1 and SiLU(z) <= max(z, 0.279)), so the cast never saturates.  Weights are
+// per-output-channel e4m3 ([n] fp32 dequantisation scales).  A 128-byte swizzle row holds 128 channels and one wgmma
+// consumes k = 32 (32 bytes), so the shared-memory addressing of the 16-bit kernels carries over byte for byte.
+// The e4m3 wgmma adder keeps fewer mantissa bits than fp32: each (tap, 128-channel chunk) is accumulated into a zeroed
+// partial that is added to the fp32 accumulators in registers (promotion every <= 128 k, as kr_gemm_fp8.cu does).
+// Epilogue: acc * (1/s) * w_scale[c], then the 16-bit epilogue unchanged (bias, residual, raw store, e4m3 out_norm or
+// the head's pixels).  fp16 only.
+// =============================================================================================
+template <int CIN>
+struct F8Chunks {
+  static constexpr int kChunks = (CIN + 127) / 128;
+  static constexpr int kLastK = (CIN % 128 == 0) ? 4 : (CIN % 128) / 32;   // k-steps of the last (zero-filled) chunk
+  static_assert(CIN % 32 == 0, "whole k = 32 steps");
+};
+
+// kK k-steps (k = 32 bytes each) of one chunk into the zeroed partial; a compile-time count keeps the wgmma chain
+// free of branches
+template <int NW, int kK>
+KR_DEVICE void f8_chunk_mma(float (&part)[NW / 2], uint32_t a, uint32_t a_sbo, uint32_t b) {
+#pragma unroll
+  for (int k = 0; k < kK; ++k)
+    wgmma_ss_e4m3<NW>(part, make_smem_desc(a + k * 32, 16, a_sbo), make_smem_desc(b + k * 32, 16, 1024), k != 0 ? 1 : 0);
+}
+
+// acc (channels c0 + 8 nb + 2 (lane % 4) + {0, 1}) *= (1/s) * w_scale[c]
+template <int NW>
+KR_DEVICE void f8_dequant(float (&acc)[NW / 2], const ConvParams& p, int c0, int lane) {
+#pragma unroll
+  for (int nb = 0; nb < NW / 8; ++nb) {
+    const float2 ws = __ldg(reinterpret_cast<const float2*>(p.w_scale + c0 + nb * 8 + 2 * (lane & 3)));
+#pragma unroll
+    for (int r = 0; r < 2; ++r) {
+      acc[4 * nb + 2 * r] = acc[4 * nb + 2 * r] * p.in_dequant * ws.x;
+      acc[4 * nb + 2 * r + 1] = acc[4 * nb + 2 * r + 1] * p.in_dequant * ws.y;
+    }
+  }
+}
+
+// Halo variant (conv_halo_kernel with byte elements): one item = kItemH x 16 output pixels of one frame, consumer
+// warpgroup u owns columns 8u..8u+7 as kMH m64 halves.  The halo box is {128 ch, 24 w, kItemH + 2 h}.  Registers per
+// consumer thread: kMH * N/2 accumulators + N/2 partial -> kMH = 2 for N = 96 (144), 1 for N = 192 (192).
+template <int CIN, int N>
+struct HaloF8Cfg {
+  static constexpr int kMH = N <= 96 ? 2 : 1;
+  static constexpr int kItemH = 8 * kMH;
+  static constexpr int kBoxW = 24, kBoxH = kItemH + 2;
+  static constexpr int kABytes = kBoxW * kBoxH * 128;
+  static constexpr int kAStages = 2;
+  static constexpr int kBBytes = N * 128;
+  static constexpr int kBStages = (96 * 1024) / kBBytes > 8 ? 8 : (96 * 1024) / kBBytes;
+  static constexpr int kSmemBytes = kAStages * kABytes + kBStages * kBBytes + 1024 + 512;
+  static_assert(kABytes % 1024 == 0 && kBBytes % 1024 == 0, "swizzle alignment");
+};
+
+template <int CIN, int N>
+__global__ void __launch_bounds__(kHaloThreads, 1)
+conv_f8_halo_kernel(const __grid_constant__ CUtensorMap tm_in, const __grid_constant__ CUtensorMap tm_w,
+                    const ConvParams p) {
+  using Cfg = HaloF8Cfg<CIN, N>;
+  using Ch = F8Chunks<CIN>;
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
+                                             ~static_cast<uintptr_t>(1023));
+  uint8_t* smem_a = smem;
+  uint8_t* smem_b = smem + Cfg::kAStages * Cfg::kABytes;
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem_b + Cfg::kBStages * Cfg::kBBytes);
+  uint64_t* a_full = bars;
+  uint64_t* a_empty = a_full + Cfg::kAStages;
+  uint64_t* b_full = a_empty + Cfg::kAStages;
+  uint64_t* b_empty = b_full + Cfg::kBStages;
+
+  const int warp = threadIdx.x >> 5;
+  const int lane = threadIdx.x & 31;
+  const int items_w = (p.W + 15) / 16;
+  const int items_h = (p.H + Cfg::kItemH - 1) / Cfg::kItemH;
+  const int items_per_frame = items_w * items_h;
+  const int num_items = p.T * items_per_frame;
+
+  if (threadIdx.x == 256) {
+    prefetch_tmap(&tm_in);
+    prefetch_tmap(&tm_w);
+    for (int i = 0; i < Cfg::kAStages; ++i) {
+      mbar_init(&a_full[i], 1);
+      mbar_init(&a_empty[i], 2);
+    }
+    for (int i = 0; i < Cfg::kBStages; ++i) {
+      mbar_init(&b_full[i], 1);
+      mbar_init(&b_empty[i], 2);
+    }
+    fence_barrier_init();
+  }
+  __syncthreads();
+
+  if (warp >= 8) {
+    // ===================== TMA producer =====================
+    producer_regs();
+    if (warp == 8 && elect_one()) {
+      int sa = 0, sb = 0;
+      uint32_t pa = 0, pb = 0;
+      for (int item = blockIdx.x; item < num_items; item += gridDim.x) {
+        const int t = item / items_per_frame;
+        const int rem = item % items_per_frame;
+        const int h0 = (rem / items_w) * Cfg::kItemH;
+        const int w0 = (rem % items_w) * 16;
+        for (int kt = 0; kt < p.KT; ++kt) {
+          for (int c = 0; c < Ch::kChunks; ++c) {
+            mbar_wait(&a_empty[sa], pa ^ 1);
+            mbar_expect_tx(&a_full[sa], Cfg::kABytes);
+            tma_load_4d(smem_a + sa * Cfg::kABytes, &tm_in, &a_full[sa], c * 128, w0 - 1, h0 - 1, t + kt);
+            if (++sa == Cfg::kAStages) {
+              sa = 0;
+              pa ^= 1;
+            }
+            for (int sp = 0; sp < 9; ++sp) {
+              mbar_wait(&b_empty[sb], pb ^ 1);
+              mbar_expect_tx(&b_full[sb], Cfg::kBBytes);
+              tma_load_2d(smem_b + sb * Cfg::kBBytes, &tm_w, &b_full[sb], (kt * 9 + sp) * CIN + c * 128, 0);
+              if (++sb == Cfg::kBStages) {
+                sb = 0;
+                pb ^= 1;
+              }
+            }
+          }
+        }
+      }
+    }
+    return;
+  }
+
+  // ===================== consumer warpgroup u: columns 8u..8u+7 of the item =====================
+  consumer_regs();
+  const int u = warp >> 2;
+  const bool leader = (threadIdx.x & 127) == 0;
+  const uint32_t a0 = smem_u32(smem_a), b0 = smem_u32(smem_b);
+  int sa = 0, sb = 0;
+  uint32_t pa = 0, pb = 0;
+  for (int item = blockIdx.x; item < num_items; item += gridDim.x) {
+    float acc[Cfg::kMH][N / 2];
+    float part[N / 2];
+#pragma unroll
+    for (int mh = 0; mh < Cfg::kMH; ++mh)
+#pragma unroll
+      for (int i = 0; i < N / 2; ++i) acc[mh][i] = 0.f;
+    for (int kt = 0; kt < p.KT; ++kt) {
+      for (int c = 0; c < Ch::kChunks; ++c) {
+        const bool last = c == Ch::kChunks - 1;
+        mbar_wait(&a_full[sa], pa);
+        const uint32_t a_st = a0 + sa * Cfg::kABytes;
+#pragma unroll 1
+        for (int sp = 0; sp < 9; ++sp) {
+          const int kh = sp / 3, kw = sp - kh * 3;
+          mbar_wait(&b_full[sb], pb);
+          const uint32_t b_st = b0 + sb * Cfg::kBBytes;
+          const uint32_t a_win = a_st + (kh * Cfg::kBoxW + 8 * u + kw) * 128;
+#pragma unroll
+          for (int mh = 0; mh < Cfg::kMH; ++mh) {
+            const uint32_t a_mh = a_win + mh * 8 * Cfg::kBoxW * 128;
+            wgmma_fence();
+            if (last)
+              f8_chunk_mma<N, Ch::kLastK>(part, a_mh, Cfg::kBoxW * 128, b_st);
+            else
+              f8_chunk_mma<N, 4>(part, a_mh, Cfg::kBoxW * 128, b_st);
+            wgmma_commit();
+            wgmma_wait<0>();
+            reg_fence(part);
+#pragma unroll
+            for (int i = 0; i < N / 2; ++i) acc[mh][i] += part[i];
+          }
+          if (leader) mbar_arrive(&b_empty[sb]);
+          if (++sb == Cfg::kBStages) {
+            sb = 0;
+            pb ^= 1;
+          }
+        }
+        if (leader) mbar_arrive(&a_empty[sa]);
+        if (++sa == Cfg::kAStages) {
+          sa = 0;
+          pa ^= 1;
+        }
+      }
+    }
+    const int t = item / items_per_frame;
+    const int rem = item % items_per_frame;
+#pragma unroll
+    for (int mh = 0; mh < Cfg::kMH; ++mh) {
+      int hh[2], ww[2];
+#pragma unroll
+      for (int r = 0; r < 2; ++r) {
+        const int px = mh * 64 + (warp & 3) * 16 + (lane >> 2) + 8 * r;   // pixel row of the kItemH x 8 tile
+        hh[r] = (rem / items_w) * Cfg::kItemH + (px >> 3);
+        ww[r] = (rem % items_w) * 16 + u * 8 + (px & 7);
+      }
+      f8_dequant<N>(acc[mh], p, 0, lane);
+      conv_epilogue_frag<N, false, true>(p, acc[mh], t, hh, ww, lane);
+    }
+  }
+}
+
+// Per-tap variant (conv_igemm_kernel with byte elements and one 128-channel chunk per stage).  N = 384 does not fit
+// twice in a warpgroup's registers, so there the work unit is 64 pixels (one half of the TH x TW tile, box
+// {128, TW, TH/2}) and consumer warpgroup j owns channels [192 j, 192 j + 192) of it (96 accumulators + 96 partial);
+// the epilogue completes the norm's sum of squares across the two warpgroups.  N <= 192: the unit is the whole tile
+// and each warpgroup owns one m64 half, as in conv_igemm_kernel.
+template <int CIN, int N>
+struct ConvF8Cfg {
+  static constexpr int kSplit = N > 192 ? 2 : 1;
+  static constexpr int kWN = N / kSplit;                 // channels per warpgroup = wgmma N
+  static constexpr int kUnitPx = kSplit == 2 ? 64 : 128;
+  static constexpr int kABytes = kUnitPx * 128;
+  static constexpr int kBBytes = N * 128;
+  static constexpr int kStageBytes = kABytes + kBBytes;
+  static constexpr int kStages = (200 * 1024) / kStageBytes > 8 ? 8 : (200 * 1024) / kStageBytes;
+  static constexpr int kSmemBytes = kStages * kStageBytes + 1024 + 256 + 512;
+  static_assert(kWN <= 256 && kStages >= 2, "tile does not fit");
+  static_assert(kABytes % 1024 == 0 && kBBytes % 1024 == 0, "swizzle alignment");
+};
+
+template <int CIN, int N>
+__global__ void __launch_bounds__(kConvThreads, 1)
+conv_f8_igemm_kernel(const __grid_constant__ CUtensorMap tm_in, const __grid_constant__ CUtensorMap tm_w,
+                     const ConvParams p) {
+  using Cfg = ConvF8Cfg<CIN, N>;
+  using Ch = F8Chunks<CIN>;
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
+                                             ~static_cast<uintptr_t>(1023));
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + Cfg::kStages * Cfg::kStageBytes);
+  uint64_t* full_bar = bars;
+  uint64_t* empty_bar = bars + Cfg::kStages;
+  float* red = reinterpret_cast<float*>(smem + Cfg::kStages * Cfg::kStageBytes + 256);   // [2][64] partial sums
+
+  const int warp = threadIdx.x >> 5;
+  const int lane = threadIdx.x & 31;
+  const int tiles_w = (p.W + p.TW - 1) / p.TW;
+  const int tiles_h = (p.H + p.TH - 1) / p.TH;
+  const int tiles_per_frame = tiles_w * tiles_h;
+  const int num_units = p.T * tiles_per_frame * Cfg::kSplit;
+  const int unit_h = p.TH / Cfg::kSplit;
+  const int taps = p.KT * p.KH * p.KW;
+  const int pad_h = p.KH / 2, pad_w = p.KW / 2;
+
+  if (threadIdx.x == 256) {
+    prefetch_tmap(&tm_in);
+    prefetch_tmap(&tm_w);
+    for (int i = 0; i < Cfg::kStages; ++i) {
+      mbar_init(&full_bar[i], 1);
+      mbar_init(&empty_bar[i], 2);
+    }
+    fence_barrier_init();
+  }
+  __syncthreads();
+
+  if (warp >= 8) {
+    // ===================== TMA producer =====================
+    producer_regs();
+    if (warp == 8 && elect_one()) {
+      int stage = 0;
+      uint32_t phase = 0;
+      for (int unit = blockIdx.x; unit < num_units; unit += gridDim.x) {
+        const int tile = unit / Cfg::kSplit, half = unit % Cfg::kSplit;
+        const int t = tile / tiles_per_frame;
+        const int rem = tile % tiles_per_frame;
+        const int h0 = (rem / tiles_w) * p.TH + half * unit_h;
+        const int w0 = (rem % tiles_w) * p.TW;
+        for (int tap = 0; tap < taps; ++tap) {
+          const int kt = tap / (p.KH * p.KW);
+          const int kh = (tap / p.KW) % p.KH;
+          const int kw = tap % p.KW;
+          for (int c = 0; c < Ch::kChunks; ++c) {
+            uint8_t* st = smem + stage * Cfg::kStageBytes;
+            mbar_wait(&empty_bar[stage], phase ^ 1);
+            mbar_expect_tx(&full_bar[stage], Cfg::kStageBytes);
+            tma_load_4d(st, &tm_in, &full_bar[stage], c * 128, w0 + kw - pad_w, h0 + kh - pad_h, t + kt);
+#pragma unroll
+            for (int j = 0; j < Cfg::kSplit; ++j)
+              tma_load_2d(st + Cfg::kABytes + j * Cfg::kWN * 128, &tm_w, &full_bar[stage], tap * CIN + c * 128,
+                          j * Cfg::kWN);
+            if (++stage == Cfg::kStages) {
+              stage = 0;
+              phase ^= 1;
+            }
+          }
+        }
+      }
+    }
+    return;
+  }
+
+  // ===================== consumer warpgroups =====================
+  consumer_regs();
+  const int wg = warp >> 2;
+  const bool leader = (threadIdx.x & 127) == 0;
+  const int k_stages = taps * Ch::kChunks;
+  const uint32_t smem0 = smem_u32(smem);
+  const uint32_t a_off = Cfg::kSplit == 2 ? 0 : wg * 64 * 128;
+  const uint32_t b_off = Cfg::kABytes + (Cfg::kSplit == 2 ? wg * Cfg::kWN * 128 : 0);
+  const int c0 = Cfg::kSplit == 2 ? wg * Cfg::kWN : 0;
+  int stage = 0;
+  uint32_t phase = 0;
+  for (int unit = blockIdx.x; unit < num_units; unit += gridDim.x) {
+    float acc[Cfg::kWN / 2];
+    float part[Cfg::kWN / 2];
+#pragma unroll
+    for (int i = 0; i < Cfg::kWN / 2; ++i) acc[i] = 0.f;
+    int c = 0;
+    for (int ks = 0; ks < k_stages; ++ks) {
+      mbar_wait(&full_bar[stage], phase);
+      const uint32_t st = smem0 + stage * Cfg::kStageBytes;
+      wgmma_fence();
+      if (c == Ch::kChunks - 1)
+        f8_chunk_mma<Cfg::kWN, Ch::kLastK>(part, st + a_off, 1024, st + b_off);
+      else
+        f8_chunk_mma<Cfg::kWN, 4>(part, st + a_off, 1024, st + b_off);
+      wgmma_commit();
+      wgmma_wait<0>();
+      reg_fence(part);
+      if (leader) mbar_arrive(&empty_bar[stage]);
+#pragma unroll
+      for (int i = 0; i < Cfg::kWN / 2; ++i) acc[i] += part[i];
+      if (++c == Ch::kChunks) c = 0;
+      if (++stage == Cfg::kStages) {
+        stage = 0;
+        phase ^= 1;
+      }
+    }
+    const int tile = unit / Cfg::kSplit, half = unit % Cfg::kSplit;
+    const int t = tile / tiles_per_frame;
+    const int rem = tile % tiles_per_frame;
+    int hh[2], ww[2];
+#pragma unroll
+    for (int r = 0; r < 2; ++r) {
+      // pixel index within the TH x TW tile
+      const int px = half * 64 + (Cfg::kSplit == 2 ? 0 : wg * 64) + (warp & 3) * 16 + (lane >> 2) + 8 * r;
+      hh[r] = (rem / tiles_w) * p.TH + px / p.TW;
+      ww[r] = (rem % tiles_w) * p.TW + px % p.TW;
+    }
+    f8_dequant<Cfg::kWN>(acc, p, c0, lane);
+    conv_epilogue_frag<N, false, true, Cfg::kSplit>(p, acc, t, hh, ww, lane, c0, red);
+  }
+}
+
+template <int CIN, int N, bool kHalo>
+static int launch_conv_f8(const void* in, int t_in, const void* wgt, int w_rows, const ConvParams& p,
+                          cudaStream_t stream) {
+  CUtensorMap tin, tw;
+  const uint64_t idims[4] = {static_cast<uint64_t>(CIN), static_cast<uint64_t>(p.W), static_cast<uint64_t>(p.H),
+                             static_cast<uint64_t>(t_in)};
+  const uint64_t istr[3] = {static_cast<uint64_t>(CIN), static_cast<uint64_t>(p.W) * CIN,
+                            static_cast<uint64_t>(p.H) * p.W * CIN};
+  const int taps = p.KT * p.KH * p.KW;
+  const uint64_t wdims[2] = {static_cast<uint64_t>(taps) * CIN, static_cast<uint64_t>(w_rows)};
+  const uint64_t wstr[1] = {static_cast<uint64_t>(taps) * CIN};
+  uint32_t ibox[4], wbox[2];
+  void (*kern)(const CUtensorMap, const CUtensorMap, const ConvParams);
+  int smem_bytes, units;
+  if constexpr (kHalo) {
+    using Cfg = HaloF8Cfg<CIN, N>;
+    ibox[0] = 128; ibox[1] = Cfg::kBoxW; ibox[2] = Cfg::kBoxH; ibox[3] = 1;
+    wbox[0] = 128; wbox[1] = N;
+    kern = conv_f8_halo_kernel<CIN, N>;
+    smem_bytes = Cfg::kSmemBytes;
+    units = p.T * ((p.W + 15) / 16) * ((p.H + Cfg::kItemH - 1) / Cfg::kItemH);
+  } else {
+    using Cfg = ConvF8Cfg<CIN, N>;
+    ibox[0] = 128; ibox[1] = p.TW; ibox[2] = p.TH / Cfg::kSplit; ibox[3] = 1;
+    wbox[0] = 128; wbox[1] = Cfg::kWN;
+    kern = conv_f8_igemm_kernel<CIN, N>;
+    smem_bytes = Cfg::kSmemBytes;
+    units = p.T * ((p.W + p.TW - 1) / p.TW) * ((p.H + p.TH - 1) / p.TH) * Cfg::kSplit;
+  }
+  int rc = make_tmap_u8(&tin, in, 4, idims, istr, ibox, 128);
+  if (rc != KR_OK) return rc;
+  rc = make_tmap_u8(&tw, wgt, 2, wdims, wstr, wbox, 128);
+  if (rc != KR_OK) return rc;
+  static bool attr_set = false;
+  if (!attr_set) {
+    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes);
+    if (e != cudaSuccess) {
+      set_last_error("vae_conv_fp8: cudaFuncSetAttribute failed: %s", cudaGetErrorString(e));
+      return KR_ERR_CUDA;
+    }
+    attr_set = true;
+  }
+  int grid = sm_count();
+  if (grid > units) grid = units;
+  kern<<<grid, kConvThreads, smem_bytes, stream>>>(tin, tw, p);
+  cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) {
+    set_last_error("vae_conv_fp8: launch failed: %s", cudaGetErrorString(e));
+    return KR_ERR_CUDA;
+  }
+  return KR_OK;
+}
+
+// in_fp8 = 1: e4m3 operands -> conv_f8_*; in_fp8 = 0: fp16 operands with an e4m3 out_norm (the producers of the FP8
+// convs' inputs that are not FP8 convs themselves: conv1 and the Resample convs)
+static int vae_conv_fp8(int in_fp8, int cin, int n, const void* in, int t_in, const void* wgt, int w_rows,
+                        const ConvParams& p, cudaStream_t s) {
+  const bool halo_taps = p.KH == 3 && p.KW == 3 && (p.KT == 1 || p.KT == 3) && w_rows >= n;
+  if (in_fp8) {
+    if (halo_taps && cin == 192 && n == 192) return launch_conv_f8<192, 192, true>(in, t_in, wgt, w_rows, p, s);
+    if (halo_taps && cin == 96 && n == 96) return launch_conv_f8<96, 96, true>(in, t_in, wgt, w_rows, p, s);
+    if (cin == 384 && n == 384) return launch_conv_f8<384, 384, false>(in, t_in, wgt, w_rows, p, s);
+    if (cin == 192 && n == 384) return launch_conv_f8<192, 384, false>(in, t_in, wgt, w_rows, p, s);
+    if (cin == 96 && n == 16) return launch_conv_f8<96, 16, false>(in, t_in, wgt, w_rows, p, s);
+  } else {
+    if (halo_taps && cin == 384 && n == 192) return launch_conv_halo<384, 192, false, true>(in, t_in, wgt, w_rows, p, s);
+    if (halo_taps && cin == 192 && n == 96) return launch_conv_halo<192, 96, false, true>(in, t_in, wgt, w_rows, p, s);
+    if (cin == 64 && n == 384) return launch_conv<64, 384, false, true>(in, t_in, wgt, w_rows, p, s);
+  }
+  set_last_error("vae_conv_fp8: unsupported configuration in_fp8=%d cin=%d n=%d taps=%dx%dx%d", in_fp8, cin, n, p.KT,
+                 p.KH, p.KW);
+  return KR_ERR_UNSUPPORTED_SHAPE;
+}
+
 // ---------------------------------------------------------------------------
 // RMS_norm (per pixel over C) * sqrt(C) * gamma -> optional SiLU; channels-last rows.
 // One warp per pixel.  (vae.py:39-54; used where the producer is not a conv epilogue.)
+// kF8: y holds e4m3 bytes e4m3(v * q_scale) of the 16-bit result v (the FP8 tier's conv input).
 // ---------------------------------------------------------------------------
-template <bool kBf16>
+template <bool kBf16, bool kF8 = false>
 __global__ void rmsnorm_silu_kernel(const uint16_t* __restrict__ x, uint16_t* __restrict__ y,
                                     const uint16_t* __restrict__ gamma, long pixels, int C,
-                                    float scale, int do_silu) {
+                                    float scale, int do_silu, float q_scale) {
   const long pix = static_cast<long>(blockIdx.x) * (blockDim.x >> 5) + (threadIdx.x >> 5);
   if (pix >= pixels) return;
   const int lane = threadIdx.x & 31;
@@ -646,8 +1089,13 @@ __global__ void rmsnorm_silu_kernel(const uint16_t* __restrict__ x, uint16_t* __
     float a = rnd16<kBf16>(v[n] * inv);
     a = rnd16<kBf16>(rnd16<kBf16>(a * scale) * load16<kBf16>(gamma + c));
     if (do_silu) a = a / (1.0f + __expf(-a));
-    const uint32_t pk = pack16<kBf16>(a, 0.f);
-    yr[c] = static_cast<uint16_t>(pk & 0xffff);
+    if constexpr (kF8) {
+      reinterpret_cast<uint8_t*>(y)[pix * C + c] =
+          __nv_cvt_float_to_fp8(rnd16<kBf16>(a) * q_scale, __NV_SATFINITE, __NV_E4M3);
+    } else {
+      const uint32_t pk = pack16<kBf16>(a, 0.f);
+      yr[c] = static_cast<uint16_t>(pk & 0xffff);
+    }
     ++n;
   }
 }
@@ -664,14 +1112,34 @@ int vae_rmsnorm_silu(int dtype, const void* x, void* y, const void* gamma, long 
   if (dtype == 0)
     rmsnorm_silu_kernel<true><<<grid, wpb * 32, 0, stream>>>(
         static_cast<const uint16_t*>(x), static_cast<uint16_t*>(y),
-        static_cast<const uint16_t*>(gamma), pixels, C, scale, do_silu);
+        static_cast<const uint16_t*>(gamma), pixels, C, scale, do_silu, 0.f);
   else
     rmsnorm_silu_kernel<false><<<grid, wpb * 32, 0, stream>>>(
         static_cast<const uint16_t*>(x), static_cast<uint16_t*>(y),
-        static_cast<const uint16_t*>(gamma), pixels, C, scale, do_silu);
+        static_cast<const uint16_t*>(gamma), pixels, C, scale, do_silu, 0.f);
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) {
     set_last_error("vae_rmsnorm_silu: launch failed: %s", cudaGetErrorString(e));
+    return KR_ERR_CUDA;
+  }
+  return KR_OK;
+}
+
+// RMS_norm + SiLU with an e4m3 output (the FP8 tier's producer after the middle attention block), fp16 only
+static int vae_rmsnorm_silu_fp8(const void* x, void* y, const void* gamma, long pixels, int C, float q_scale,
+                                cudaStream_t stream) {
+  if (C > 384 || C <= 0 || pixels <= 0) {
+    set_last_error("vae_rmsnorm_silu_fp8: unsupported C=%d", C);
+    return KR_ERR_UNSUPPORTED_SHAPE;
+  }
+  const int wpb = 8;
+  const unsigned grid = static_cast<unsigned>((pixels + wpb - 1) / wpb);
+  rmsnorm_silu_kernel<false, true><<<grid, wpb * 32, 0, stream>>>(
+      static_cast<const uint16_t*>(x), static_cast<uint16_t*>(y), static_cast<const uint16_t*>(gamma), pixels, C,
+      sqrtf(static_cast<float>(C)), 1, q_scale);
+  cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) {
+    set_last_error("vae_rmsnorm_silu_fp8: launch failed: %s", cudaGetErrorString(e));
     return KR_ERR_CUDA;
   }
   return KR_OK;
@@ -904,3 +1372,54 @@ int frames_to_rgb8(const float* pixels, uint8_t* rgb, int frames, int height, in
 }
 
 }  // namespace kr
+
+// ---------------------------------------------------------------------------------------------
+// C ABI of the FP8 tier (include/krea_b200_vae_fp8.h).  Defined here rather than in kr_api.cu so that the API layer
+// links without the kernels (the launch-recording build of tests/test_block_fwd_cpu.py).
+// ---------------------------------------------------------------------------------------------
+#define KR_VAE_F8_REQUIRE(cond, msg)               \
+  do {                                             \
+    if (!(cond)) {                                 \
+      kr::set_last_error("%s: %s", __func__, msg); \
+      return KR_ERR_INVALID_ARG;                   \
+    }                                              \
+  } while (0)
+
+extern "C" int kr_vae_conv_fp8(int in_fp8, int cin, int n, const void* in, int t_in, const void* weight,
+                               const float* w_scale, float in_scale, int w_rows, const void* bias, int cout, int T,
+                               int H, int W, int tile_w, int tile_h, int kt, int kh, int kw, void* out_raw,
+                               long raw_pix, long raw_frame, void* out_norm, long norm_pix, long norm_frame,
+                               float norm_q_scale, const void* gamma, const void* residual, long res_pix,
+                               long res_frame, float* out_pix, void* stream) {
+  KR_VAE_F8_REQUIRE(in && weight, "null input/weight");
+  KR_VAE_F8_REQUIRE(in_fp8 == 0 || in_fp8 == 1, "in_fp8 must be 0 or 1");
+  KR_VAE_F8_REQUIRE(out_raw || out_norm || out_pix, "no output requested");
+  KR_VAE_F8_REQUIRE(in_fp8 || out_norm, "16-bit input without an e4m3 out_norm: use kr_vae_conv3d");
+  KR_VAE_F8_REQUIRE(!in_fp8 || (w_scale && reinterpret_cast<uintptr_t>(w_scale) % 8 == 0),
+                    "e4m3 weights need 8-byte aligned [n] channel scales");
+  KR_VAE_F8_REQUIRE(!in_fp8 || (std::isfinite(in_scale) && in_scale > 0.f), "in_scale must be finite and > 0");
+  KR_VAE_F8_REQUIRE(!out_norm || (gamma && std::isfinite(norm_q_scale) && norm_q_scale > 0.f),
+                    "e4m3 out_norm needs gamma and a finite norm_q_scale > 0");
+  KR_VAE_F8_REQUIRE(tile_w * tile_h == 128 && T > 0 && H > 0 && W > 0, "bad geometry");
+  KR_VAE_F8_REQUIRE((kt == 1 || kt == 3) && (kh == 1 || kh == 3) && (kw == 1 || kw == 3), "taps must be 1 or 3");
+  KR_VAE_F8_REQUIRE(t_in >= T + kt - 1, "input holds too few frames");
+  kr::ConvParams p;
+  p.T = T; p.H = H; p.W = W; p.TW = tile_w; p.TH = tile_h; p.KT = kt; p.KH = kh; p.KW = kw;
+  p.cout = cout;
+  p.out_raw = out_raw; p.raw_pix = raw_pix; p.raw_frame = raw_frame;
+  p.out_norm = out_norm; p.norm_pix = norm_pix; p.norm_frame = norm_frame;
+  p.out_pix = out_pix; p.bias = bias;
+  p.residual = residual; p.res_pix = res_pix; p.res_frame = res_frame;
+  p.gamma = gamma; p.norm_scale = sqrtf(static_cast<float>(cout)); p.sub2 = 0;
+  p.norm_q_scale = norm_q_scale;
+  p.in_dequant = in_fp8 ? 1.0f / in_scale : 0.f;
+  p.w_scale = w_scale;
+  return kr::vae_conv_fp8(in_fp8, cin, n, in, t_in, weight, w_rows, p, static_cast<cudaStream_t>(stream));
+}
+
+extern "C" int kr_vae_rmsnorm_silu_fp8(const void* x, void* y, const void* gamma, long pixels, int C, float q_scale,
+                                       void* stream) {
+  KR_VAE_F8_REQUIRE(x && y && gamma, "null pointer");
+  KR_VAE_F8_REQUIRE(std::isfinite(q_scale) && q_scale > 0.f, "q_scale must be finite and > 0");
+  return kr::vae_rmsnorm_silu_fp8(x, y, gamma, pixels, C, q_scale, static_cast<cudaStream_t>(stream));
+}

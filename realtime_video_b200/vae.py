@@ -20,6 +20,7 @@ arithmetically identical to the reference's frame-by-frame loop because every co
 from __future__ import annotations
 
 import math
+import os
 from typing import List, Optional
 
 import torch
@@ -157,6 +158,9 @@ class _Conv:
         self.weight, self.bias = weight, bias
         self.cin, self.n, self.cout, self.taps = cin_pad, n_pad, cout, taps
         self.buf: Optional[torch.Tensor] = None     # [kt-1 + Tmax, H, W, cin]
+        # FP8 tier: e4m3 weight (replaces ``weight``), fp32 channel scales [n] and the static activation scale of buf
+        self.w_scale: Optional[torch.Tensor] = None
+        self.in_scale: Optional[float] = None
 
 
 def _prep_conv(w: torch.Tensor, b: torch.Tensor, dtype, device, cin_pad=None, n_pad=None) -> _Conv:
@@ -170,6 +174,38 @@ def _prep_conv(w: torch.Tensor, b: torch.Tensor, dtype, device, cin_pad=None, n_
     bp = torch.zeros(max(n_pad, 32), dtype=dtype, device=device)
     bp[:cout] = b.to(device=device, dtype=dtype)
     return _Conv(wp.reshape(n_pad, kt * kh * kw * cin_pad).contiguous(), bp, cin_pad, n_pad, cout, (kt, kh, kw))
+
+
+# ---------------------------------------------------------------------------------------------
+# FP8 tier (quant = "fp8"): the convs whose input is a normalised tensor read e4m3 activations and weights
+# ---------------------------------------------------------------------------------------------
+E4M3_MAX = 448.0
+SILU_NEG_BOUND = 0.28          # |SiLU(z)| <= max(|z|, 0.2785) for every z
+
+
+def fp8_input_scale(gamma: torch.Tensor) -> float:
+    """Static e4m3 scale of the input of a conv fed by SiLU(RMS_norm(x) * sqrt(C) * gamma): an RMS-normalised pixel
+    is a unit vector times sqrt(C), so every input element is bounded by sqrt(C) * max|gamma| (SiLU only shrinks
+    positive values, and its negative range ends at -0.2785).  s = 448 / that bound never saturates and depends only
+    on the weights: no amax pass, deterministic, and the cached frames stay valid from block to block."""
+    g = gamma.detach().float().abs().max().item()
+    bound = max(math.sqrt(gamma.numel()) * g, SILU_NEG_BOUND)
+    return float(torch.tensor(E4M3_MAX / bound, dtype=torch.float32).item())
+
+
+def fp8_quantize_weight(w: torch.Tensor):
+    """Per-output-channel e4m3 weights: w [n, K] -> (w_q e4m3 [n, K], scale fp32 [n]) with w ~ w_q * scale[:, None],
+    scale = amax_row / 448 (1 for all-zero padding rows)."""
+    w32 = w.detach().float()
+    amax = w32.abs().amax(dim=1)
+    scale = torch.where(amax > 0, amax / E4M3_MAX, torch.ones_like(amax))
+    w_q = (w32 / scale[:, None]).clamp(-E4M3_MAX, E4M3_MAX).to(torch.float8_e4m3fn)
+    return w_q.contiguous(), scale.contiguous()
+
+
+def _to_fp8(c: _Conv, gamma: torch.Tensor) -> None:
+    c.weight, c.w_scale = fp8_quantize_weight(c.weight)
+    c.in_scale = fp8_input_scale(gamma)
 
 
 def _vae_attention(b, x):
@@ -252,8 +288,11 @@ class DecoderEngine(_StreamLedger):
     MAX_CHUNK = 3          # latent frames per launch sequence
 
     def __init__(self, decoder: VAEDecoder3d, conv2: nn.Module, mean: torch.Tensor, std: torch.Tensor,
-                 single_mode: bool = False):
+                 single_mode: bool = False, quant: Optional[str] = None):
         self.decoder, self.conv2, self.mean, self.std = decoder, conv2, mean, std
+        # None: fp16 / bf16 everywhere; "fp8": residual.2 / residual.6 of every ResidualBlock and head.2 run on e4m3
+        # inputs and weights (fp16 only).  Part of the prepared-weights key: switching rebuilds the buffers.
+        self.quant = quant
         # single_mode: semantics of demo_utils/vae.py (VAEDecoderWrapperSingle), see decode_single
         self.single_mode = single_mode
         self._key = None
@@ -261,7 +300,11 @@ class DecoderEngine(_StreamLedger):
 
     # -- weight preparation ---------------------------------------------------------------
     def _prepare(self, dtype, device, H, W):
-        key = (dtype, str(device), H, W, _weights_tag(self.decoder.conv1.weight))
+        if self.quant not in (None, "fp8"):
+            raise ValueError(f"VAE decoder quant must be 'fp8' or None, got {self.quant!r}")
+        if self.quant == "fp8" and dtype != torch.float16:
+            raise ValueError(f"the FP8 VAE tier runs in float16, got {dtype}")
+        key = (dtype, str(device), H, W, _weights_tag(self.decoder.conv1.weight), self.quant)
         if self._key == key:
             return
         d = self.decoder
@@ -297,6 +340,12 @@ class DecoderEngine(_StreamLedger):
                 self.blocks.append(e)
         self.g_head = g(d.head[0])
         self.head = pc(d.head[2], n_pad=16)
+        if self.quant == "fp8":
+            for b in self.blocks:
+                if b["kind"] == "res":
+                    _to_fp8(b["c1"], b["g1"])
+                    _to_fp8(b["c2"], b["g2"])
+            _to_fp8(self.head, self.g_head)
         self._key = key
         self._alloc(H, W)
 
@@ -307,7 +356,8 @@ class DecoderEngine(_StreamLedger):
         T = self.MAX_CHUNK
 
         def buf(conv: _Conv, t, h, w):
-            conv.buf = torch.zeros(conv.taps[0] - 1 + t, h, w, conv.cin, dtype=dt, device=dev)
+            conv.buf = torch.zeros(conv.taps[0] - 1 + t, h, w, conv.cin, device=dev,
+                                   dtype=torch.float8_e4m3fn if conv.in_scale is not None else dt)
 
         buf(self.conv1, T, H, W)
         h, w, t = H, W, T
@@ -362,14 +412,21 @@ class DecoderEngine(_StreamLedger):
         self.initialised = True
 
     # -- one conv with fused epilogue --------------------------------------------------------
-    def _conv(self, c: _Conv, T, src: Optional[torch.Tensor] = None, **kw):
+    def _conv(self, c: _Conv, T, src: Optional[torch.Tensor] = None, norm_scale: Optional[float] = None, **kw):
         x = c.buf if src is None else src
         H, W = x.shape[1], x.shape[2]
-        ops.vae_conv(x, c.weight, c.bias, n=c.n, cout=c.cout, T=T, taps=c.taps, tile=_tile_for(H, W), **kw)
+        out_norm = kw.get("out_norm")
+        if x.dtype == torch.float8_e4m3fn or (out_norm is not None and out_norm.dtype == torch.float8_e4m3fn):
+            # FP8 tier: an e4m3 conv, or a 16-bit conv writing the e4m3 input of the next one
+            ops.vae_conv_fp8(x, c.weight, c.bias, n=c.n, cout=c.cout, T=T, taps=c.taps, tile=_tile_for(H, W),
+                             w_scale=c.w_scale, in_scale=c.in_scale, norm_scale=norm_scale, **kw)
+        else:
+            ops.vae_conv(x, c.weight, c.bias, n=c.n, cout=c.cout, T=T, taps=c.taps, tile=_tile_for(H, W), **kw)
         if src is None and c.taps[0] == 3:
             # roll: the last two input frames become the cache (frames = rows of a [frames, H*W*C] view; the
-            # in-place row shift is overlap-safe, so T = 1 needs no temporary)
-            ops.kv_roll(c.buf.view(c.buf.shape[0], -1), 0, T, 2)
+            # in-place row shift is overlap-safe, so T = 1 needs no temporary); e4m3 buffers move as 16-bit pairs
+            buf = c.buf.view(torch.float16) if c.buf.dtype == torch.float8_e4m3fn else c.buf
+            ops.kv_roll(buf.view(buf.shape[0], -1), 0, T, 2)
 
     def _new(self, t, h, w, c):
         return torch.empty(t, h, w, c, dtype=self.dtype, device=self.device)
@@ -398,7 +455,7 @@ class DecoderEngine(_StreamLedger):
         # conv1 -> raw x (residual stream) + normalised input of middle.0.conv1
         x = self._new(T, h, w, c1.cout)
         g, nxt = blocks[0]["g1"], blocks[0]["c1"]
-        self._conv(c1, T, out_raw=x, out_norm=nxt.buf[2:2 + T], gamma=g)
+        self._conv(c1, T, out_raw=x, out_norm=nxt.buf[2:2 + T], gamma=g, norm_scale=nxt.in_scale)
 
         for i, b in enumerate(blocks):
             if b["kind"] == "res":
@@ -407,17 +464,21 @@ class DecoderEngine(_StreamLedger):
                 if b["sc"] is not None:
                     res = self._new(T, h, w, b["cout"])
                     self._conv(b["sc"], T, src=x, out_raw=res)
-                self._conv(ca, T, out_norm=cb.buf[2:2 + T], gamma=b["g2"])
+                self._conv(ca, T, out_norm=cb.buf[2:2 + T], gamma=b["g2"], norm_scale=cb.in_scale)
                 g, nxt = next_gamma(i)
                 need_raw = nxt is not self.head          # the head only needs the normalised tensor
                 xo = self._new(T, h, w, b["cout"]) if need_raw else None
                 self._conv(cb, T, residual=res, out_raw=xo,
-                           out_norm=nxt.buf[2:2 + T] if g is not None else None, gamma=g)
+                           out_norm=nxt.buf[2:2 + T] if g is not None else None, gamma=g,
+                           norm_scale=nxt.in_scale if g is not None else None)
                 x = xo
             elif b["kind"] == "attn":
                 x = self._attention(b, x)
                 nb = blocks[i + 1]
-                ops.vae_rmsnorm_silu(x, nb["g1"], nb["c1"].buf[2:2 + T])
+                if nb["c1"].in_scale is not None:
+                    ops.vae_rmsnorm_silu_fp8(x, nb["g1"], nb["c1"].buf[2:2 + T], nb["c1"].in_scale)
+                else:
+                    ops.vae_rmsnorm_silu(x, nb["g1"], nb["c1"].buf[2:2 + T])
             else:  # Resample
                 C = b["C"]
                 if b["mode"] == "upsample3d":
@@ -458,7 +519,7 @@ class DecoderEngine(_StreamLedger):
                 cv = b["conv"]
                 x = self._new(T, h, w, cv.cout)
                 g, nxt = next_gamma(i)
-                self._conv(cv, T, src=up, out_raw=x, out_norm=nxt.buf[2:2 + T], gamma=g)
+                self._conv(cv, T, src=up, out_raw=x, out_norm=nxt.buf[2:2 + T], gamma=g, norm_scale=nxt.in_scale)
         # head conv -> clamped fp32 pixels [T, 3, H, W]
         pix = torch.empty(T, 3, h, w, dtype=torch.float32, device=self.device)
         self._conv(self.head, T, out_pix=pix)
@@ -480,6 +541,10 @@ class DecoderEngine(_StreamLedger):
         zt = z[0]
         dtype = zt.dtype if zt.dtype in (torch.float16, torch.bfloat16) else torch.float16
         self._prepare(dtype, zt.device, zt.shape[-2], zt.shape[-1])
+        if feat_cache is not None and any(
+                c is not None and m is not None and (c.dtype == torch.float8_e4m3fn) != (m.dtype == torch.float8_e4m3fn)
+                for c, m in zip(feat_cache, self._views())):
+            feat_cache = None        # a cache of the other tier (quant was switched): its values do not carry over
         self.import_cache(feat_cache)
         zt = zt.to(dtype)
         outs = []
@@ -548,6 +613,10 @@ def _(z, first, handle):
 # ---------------------------------------------------------------------------------------------
 # the reference-facing wrappers
 # ---------------------------------------------------------------------------------------------
+def _default_quant() -> Optional[str]:
+    return "fp8" if os.environ.get("KR_VAE_FP8", "0") not in ("", "0") else None
+
+
 class VAEDecoderWrapper(nn.Module):
     """demo_utils/vae_block3.py:177-230: ``forward(z[1,T,16,h,w], *feat_cache) ->
     (pixels [1,T',3,H,W] fp32 in [-1,1], feat_cache)``.  The cache list entries are this
@@ -562,6 +631,9 @@ class VAEDecoderWrapper(nn.Module):
         self.conv2 = CausalConv3d(self.z_dim, self.z_dim, 1)
         self._engine: Optional[DecoderEngine] = None
         self._handle = _register_decoder(self)      # id of this module for the opaque torch.compile op
+        # "fp8": the FP8 (e4m3) tier of the normalised-input convs (fp16 only); KR_VAE_FP8=1 turns it on by default.
+        # Switching the tier rebuilds the engine's buffers: the next call starts a new stream.
+        self.quant: Optional[str] = _default_quant()
 
     def __setstate__(self, state):                  # deepcopy / unpickle (release_server.py:111-119): own handle, own engine
         super().__setstate__(state)
@@ -580,7 +652,7 @@ class VAEDecoderWrapper(nn.Module):
 
     def _decode(self, z: torch.Tensor, feat_cache):
         eng = self.engine
-        eng.mean, eng.std = self.mean, self.std
+        eng.mean, eng.std, eng.quant = self.mean, self.std, self.quant
         return eng.decode(z, feat_cache)
 
     def forward(self, z: torch.Tensor, *feat_cache):
@@ -611,6 +683,7 @@ class VAEDecoderWrapperSingle(nn.Module):
         self.z_dim = 16
         self.conv2 = CausalConv3d(self.z_dim, self.z_dim, 1)
         self._engine: Optional[DecoderEngine] = None
+        self.quant: Optional[str] = _default_quant()      # as VAEDecoderWrapper.quant
 
     def _apply(self, fn, *a, **k):
         self._engine = None
@@ -620,6 +693,7 @@ class VAEDecoderWrapperSingle(nn.Module):
     def forward(self, z: torch.Tensor, is_first_frame: torch.Tensor, *feat_cache):
         if self._engine is None:
             self._engine = DecoderEngine(self.decoder, self.conv2, self.mean, self.std, single_mode=True)
+        self._engine.quant = self.quant
         return self._engine.decode_single(z, is_first_frame, list(feat_cache))
 
 
