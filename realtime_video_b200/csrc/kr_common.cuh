@@ -196,6 +196,11 @@ KR_DEVICE void reg_fence(float (&d)[N]) {
 // consumer warpgroups take them (3 warpgroups: 128 x 40 + 256 x 232 <= 64 K)
 KR_DEVICE void producer_regs() { asm volatile("setmaxnreg.dec.sync.aligned.u32 40;"); }
 KR_DEVICE void consumer_regs() { asm volatile("setmaxnreg.inc.sync.aligned.u32 232;"); }
+// the same with another split (kernels whose producer warpgroup also runs an epilogue)
+template <int R>
+KR_DEVICE void producer_regs_n() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
+template <int R>
+KR_DEVICE void consumer_regs_n() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
 // named barrier over `count` threads (the consumer warpgroups of a kernel)
 KR_DEVICE void named_bar_sync(int id, int count) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory");

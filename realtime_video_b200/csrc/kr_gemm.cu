@@ -18,6 +18,13 @@
 //                 full/empty ring; it hands most of its registers to the consumers (setmaxnreg)
 // BLOCK_N is a template parameter (the wgmma instruction encodes N); gemm_tn_kernel serves the fixed widths
 // 32..256, gemm_flex_kernel the wave-fitted widths 96..256 whose last column tile may be narrower.
+//
+// 16-bit epilogues with epilogue warps (kEpiWarps, KR_GEMM_EPI_WARPS=1, the default): the epilogue is split at its
+// first rounding point.  A consumer warpgroup writes rnd16(acc + bias) of its 64-row slice into its own shared C
+// buffer, arrives on c_full and goes on with the next tile's mainloop; warps 9..11 (idle otherwise) wait on c_full,
+// apply the rest of the chain (GELU-tanh / per-frame gate / residual / multiply, the split output), store, and arrive
+// on c_empty, which the consumer waits on before it writes the buffer again.  Rounding an already 16-bit value is
+// exact, so the outputs are bit-identical to the in-register epilogue, which EPI_F32 and KR_GEMM_EPI_WARPS=0 keep.
 #include "kr_common.cuh"
 #include "kr_gemm_epi.cuh"
 #include "kr_ops.h"
@@ -32,31 +39,151 @@ static constexpr int BLOCK_K = 64;   // 64 x 16-bit = 128 B = one swizzle row
 static constexpr int kNumThreads = 384;
 static constexpr int kSmemBudget = 227 * 1024;
 
-template <int BLOCK_N>
+static constexpr int kEpiThreads = 96;   // warps 9..11
+
+// kEpiWarps: the epilogue-warp split above, with a shared C buffer per consumer warpgroup (64 rows, 16-bit, row
+// pitch padded by 16 B so that the fragment stores of a warp hit 32 distinct banks) instead of the per-warp transpose
+// scratch; the stage count is whatever the rest of the budget holds (3 at BLOCK_N = 256, 4 without the C buffers).
+template <int BLOCK_N, bool kEpiWarps = false>
 struct GemmCfg {
   static constexpr int kABytes = BLOCK_M * BLOCK_K * 2;
   static constexpr int kBBytes = BLOCK_N * BLOCK_K * 2;
   static constexpr int kStageBytes = kABytes + kBBytes;
-  static constexpr int kScrBytes = 8 * kEpiScrFloats * 4;
-  static constexpr int kFit = (kSmemBudget - kScrBytes - 2048) / kStageBytes;
+  static constexpr int kCPitch = BLOCK_N * 2 + 16;
+  static constexpr int kCHalfBytes = 64 * kCPitch;
+  static constexpr int kEpiBytes = kEpiWarps ? 2 * kCHalfBytes : 8 * kEpiScrFloats * 4;
+  static constexpr int kFit = (kSmemBudget - kEpiBytes - 2048) / kStageBytes;
   static constexpr int kStages = kFit > 8 ? 8 : kFit;
-  static constexpr int kSmemBytes = kStages * kStageBytes + kScrBytes + 1024 /*align*/ + 256 /*barriers*/;
+  static constexpr int kSmemBytes = kStages * kStageBytes + kEpiBytes + 1024 /*align*/ + 256 /*barriers*/;
   static_assert(kStages >= 2, "pipeline needs >= 2 stages");
+  static_assert((2 * kStages + 4) * 8 <= 256, "barrier area");
 };
 
-template <int BLOCK_N, bool kBf16, int kEpi>
+// Consumer half of the split epilogue: the warp's accumulator fragment (rows 16 * (warp & 3) + [0, 16) of the
+// warpgroup's slice) -> rnd16(acc + bias) -> the C buffer.  Columns >= n_valid (a multiple of 32) are not written.
+template <int BN, bool kBf16>
+KR_DEVICE void gemm_frag_to_ctile(const float (&acc)[BN / 2], uint8_t* ct, int col_base, int n_valid,
+                                  const GemmParams& p) {
+  constexpr int kPitch = GemmCfg<BN, true>::kCPitch;
+  const int lane = threadIdx.x & 31, c2 = 2 * (lane & 3);
+  uint8_t* d = ct + (((threadIdx.x >> 5) & 3) * 16 + (lane >> 2)) * kPitch + c2 * 2;
+  auto pack = [](float x, float y) { return kBf16 ? pack_bf16x2(x, y) : pack_f16x2(x, y); };
+  const uint32_t* bias = reinterpret_cast<const uint32_t*>(reinterpret_cast<const uint16_t*>(p.bias) + col_base + c2);
+  if (p.bias != nullptr) {
+#pragma unroll
+    for (int j = 0; j < BN / 8; ++j) {
+      if (j * 8 < n_valid) {
+        const float2 b = kBf16 ? unpack_bf16x2(__ldg(bias + 4 * j)) : unpack_f16x2(__ldg(bias + 4 * j));
+        *reinterpret_cast<uint32_t*>(d + j * 16) = pack(acc[4 * j] + b.x, acc[4 * j + 1] + b.y);
+        *reinterpret_cast<uint32_t*>(d + 8 * kPitch + j * 16) = pack(acc[4 * j + 2] + b.x, acc[4 * j + 3] + b.y);
+      }
+    }
+  } else {
+#pragma unroll
+    for (int j = 0; j < BN / 8; ++j) {
+      if (j * 8 < n_valid) {
+        *reinterpret_cast<uint32_t*>(d + j * 16) = pack(acc[4 * j], acc[4 * j + 1]);
+        *reinterpret_cast<uint32_t*>(d + 8 * kPitch + j * 16) = pack(acc[4 * j + 2], acc[4 * j + 3]);
+      }
+    }
+  }
+}
+
+// Epilogue-warp half: one C buffer (output rows row0 + [0, 64), columns col_base + [0, n_valid)) -> the rest of
+// gemm_epilogue_row's chain, applied to the already rounded values with the same expressions in the same order ->
+// 16-byte stores.  kU vectors per thread are loaded (C buffer, gate, residual) before any is stored, so that their
+// global loads overlap although the output may alias the residual.
+template <int BN, bool kBf16, int kEpi>
+KR_DEVICE void gemm_ctile_epilogue(const uint8_t* ct, int row0, int col_base, int n_valid, const GemmParams& p,
+                                   int et) {
+  constexpr int kPitch = GemmCfg<BN, true>::kCPitch, kVec = BN / 8, kTotal = 64 * kVec, kU = 2;
+  constexpr bool kRes = kEpi == EPI_BIAS_GATE_RES || kEpi == EPI_BIAS_RES || kEpi == EPI_MUL;
+  auto rnd = [](float x) -> float {
+    return kBf16 ? __bfloat162float(__float2bfloat16_rn(x)) : __half2float(__float2half_rn(x));
+  };
+  auto unpack = [](uint32_t w) { return kBf16 ? unpack_bf16x2(w) : unpack_f16x2(w); };
+  auto pack = [](float x, float y) { return kBf16 ? pack_bf16x2(x, y) : pack_f16x2(x, y); };
+  for (int i0 = et; i0 < kTotal; i0 += kEpiThreads * kU) {
+    uint4 c[kU], r[kU], g[kU];
+    int row[kU], col[kU];
+    bool ok[kU];
+#pragma unroll
+    for (int u = 0; u < kU; ++u) {
+      const int i = i0 + u * kEpiThreads, tr = i / kVec, cv = i - tr * kVec;
+      row[u] = row0 + tr;
+      col[u] = col_base + cv * 8;
+      ok[u] = i < kTotal && row[u] < p.M && cv * 8 < n_valid;
+      if (ok[u]) {
+        c[u] = *reinterpret_cast<const uint4*>(ct + tr * kPitch + cv * 16);
+        if constexpr (kRes)
+          r[u] = *reinterpret_cast<const uint4*>(reinterpret_cast<const uint16_t*>(p.residual) +
+                                                 static_cast<size_t>(row[u]) * p.ldr + col[u]);
+        if constexpr (kEpi == EPI_BIAS_GATE_RES) {
+          const int gi = (row[u] + p.row_offset) / p.rows_per_gate;
+          g[u] = __ldg(reinterpret_cast<const uint4*>(reinterpret_cast<const uint16_t*>(p.gate) +
+                                                      static_cast<size_t>(gi) * p.gate_stride + col[u]));
+        }
+      }
+    }
+#pragma unroll
+    for (int u = 0; u < kU; ++u) {
+      if (!ok[u]) continue;
+      uint4 w = c[u];
+      if constexpr (kEpi != EPI_BIAS) {
+        const uint32_t cw[4] = {c[u].x, c[u].y, c[u].z, c[u].w};
+        const uint32_t rw[4] = {r[u].x, r[u].y, r[u].z, r[u].w};
+        const uint32_t gw[4] = {g[u].x, g[u].y, g[u].z, g[u].w};
+        uint32_t ow[4];
+#pragma unroll
+        for (int h = 0; h < 4; ++h) {
+          float2 v = unpack(cw[h]);
+          if constexpr (kEpi == EPI_BIAS_GELU) {
+            v.x = gelu_tanh(v.x);
+            v.y = gelu_tanh(v.y);
+          }
+          if constexpr (kEpi == EPI_BIAS_GATE_RES) {
+            const float2 f = unpack(gw[h]);
+            v.x = rnd(v.x * f.x);
+            v.y = rnd(v.y * f.y);
+          }
+          if constexpr (kRes) {
+            const float2 f = unpack(rw[h]);
+            if constexpr (kEpi == EPI_MUL) {
+              v.x = f.x * v.x;
+              v.y = f.y * v.y;
+            } else {
+              v.x = f.x + v.x;
+              v.y = f.y + v.y;
+            }
+          }
+          ow[h] = pack(v.x, v.y);
+        }
+        w = make_uint4(ow[0], ow[1], ow[2], ow[3]);
+      }
+      uint16_t* o = (p.out2 != nullptr && col[u] >= p.n_split)
+          ? reinterpret_cast<uint16_t*>(p.out2) + static_cast<size_t>(row[u]) * p.ldc2 + (col[u] - p.n_split)
+          : reinterpret_cast<uint16_t*>(p.out) + static_cast<size_t>(row[u]) * p.ldc + col[u];
+      *reinterpret_cast<uint4*>(o) = w;
+    }
+  }
+}
+
+template <int BLOCK_N, bool kBf16, int kEpi, bool kEpiWarps>
 KR_DEVICE void gemm_body(const CUtensorMap* tmap_a, const CUtensorMap* tmap_b, const GemmParams& p) {
-  using Cfg = GemmCfg<BLOCK_N>;
+  static_assert(!(kEpiWarps && kEpi == EPI_F32), "an fp32 C tile does not fit: EPI_F32 keeps the register epilogue");
+  using Cfg = GemmCfg<BLOCK_N, kEpiWarps>;
   extern __shared__ uint8_t smem_raw[];
   // 1024 B alignment for SWIZZLE_128B tiles
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
                                              ~static_cast<uintptr_t>(1023));
   uint8_t* smem_a = smem;
   uint8_t* smem_b = smem + Cfg::kStages * Cfg::kABytes;
-  float* scratch = reinterpret_cast<float*>(smem + Cfg::kStages * Cfg::kStageBytes);
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + Cfg::kStages * Cfg::kStageBytes + Cfg::kScrBytes);
+  uint8_t* epi_smem = smem + Cfg::kStages * Cfg::kStageBytes;   // transpose scratch, or the two C buffers
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + Cfg::kStages * Cfg::kStageBytes + Cfg::kEpiBytes);
   uint64_t* full_bar = bars;                       // [kStages]
   uint64_t* empty_bar = bars + Cfg::kStages;       // [kStages]
+  uint64_t* c_full = bars + 2 * Cfg::kStages;      // [2] per consumer warpgroup (kEpiWarps)
+  uint64_t* c_empty = c_full + 2;                  // [2]
 
   const int warp = threadIdx.x >> 5;
 
@@ -72,13 +199,38 @@ KR_DEVICE void gemm_body(const CUtensorMap* tmap_a, const CUtensorMap* tmap_b, c
       mbar_init(&full_bar[i], 1);
       mbar_init(&empty_bar[i], 2);   // one arrive per consumer warpgroup
     }
+    if constexpr (kEpiWarps) {
+      for (int h = 0; h < 2; ++h) {
+        mbar_init(&c_full[h], 128);           // every thread of the consumer warpgroup
+        mbar_init(&c_empty[h], kEpiThreads);  // every epilogue thread
+      }
+    }
     fence_barrier_init();
   }
   __syncthreads();
 
   if (warp >= 8) {
-    // ===================== TMA producer (warp 8; warps 9..11 only give their registers back) =====================
-    producer_regs();
+    // ===================== TMA producer (warp 8) and, with kEpiWarps, the epilogue warps 9..11 =====================
+    if constexpr (kEpiWarps) producer_regs_n<72>();
+    else producer_regs();
+    if constexpr (kEpiWarps) {
+      if (warp >= 9) {
+        uint32_t cph = 0;
+        for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+          const int m_blk = tile % num_m;
+          const int n_blk = tile / num_m;
+          const int n_valid = (p.N - n_blk * BLOCK_N) < BLOCK_N ? (p.N - n_blk * BLOCK_N) : BLOCK_N;
+#pragma unroll 1
+          for (int h = 0; h < 2; ++h) {
+            mbar_wait(&c_full[h], cph);
+            gemm_ctile_epilogue<BLOCK_N, kBf16, kEpi>(epi_smem + h * Cfg::kCHalfBytes, m_blk * BLOCK_M + h * 64,
+                                                      n_blk * BLOCK_N, n_valid, p, threadIdx.x - 288);
+            mbar_arrive(&c_empty[h]);
+          }
+          cph ^= 1;
+        }
+      }
+    }
     if (warp == 8 && elect_one()) {
       int stage = 0;
       uint32_t phase = 0;
@@ -101,12 +253,13 @@ KR_DEVICE void gemm_body(const CUtensorMap* tmap_a, const CUtensorMap* tmap_b, c
     }
   } else {
     // ===================== consumer warpgroups =====================
-    consumer_regs();
+    if constexpr (kEpiWarps) consumer_regs_n<216>();
+    else consumer_regs();
     const int wg = warp >> 2;
     const uint32_t a_base = smem_u32(smem_a) + wg * 64 * 128, b_base = smem_u32(smem_b);
-    float* scr = scratch + warp * kEpiScrFloats;
+    float* scr = reinterpret_cast<float*>(epi_smem) + warp * kEpiScrFloats;
     int stage = 0;
-    uint32_t phase = 0;
+    uint32_t phase = 0, cph = 0;
     for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
       const int m_blk = tile % num_m;
       const int n_blk = tile / num_m;
@@ -114,45 +267,60 @@ KR_DEVICE void gemm_body(const CUtensorMap* tmap_a, const CUtensorMap* tmap_b, c
       gemm_mainloop<BLOCK_N, kBf16 ? 0 : 1>(acc, a_base, b_base, Cfg::kABytes, Cfg::kBBytes, Cfg::kStages,
                                             full_bar, empty_bar, stage, phase, 0, num_k);
       const int n_valid = (p.N - n_blk * BLOCK_N) < BLOCK_N ? (p.N - n_blk * BLOCK_N) : BLOCK_N;
-      gemm_frag_epilogue<BLOCK_N, kBf16, kEpi>(acc, scr, m_blk * BLOCK_M + wg * 64 + (warp & 3) * 16,
-                                               n_blk * BLOCK_N, n_valid, 1.0f, p);
+      if constexpr (kEpiWarps) {
+        mbar_wait(&c_empty[wg], cph ^ 1);
+        gemm_frag_to_ctile<BLOCK_N, kBf16>(acc, epi_smem + wg * Cfg::kCHalfBytes, n_blk * BLOCK_N, n_valid, p);
+        mbar_arrive(&c_full[wg]);
+        cph ^= 1;
+      } else {
+        gemm_frag_epilogue<BLOCK_N, kBf16, kEpi>(acc, scr, m_blk * BLOCK_M + wg * 64 + (warp & 3) * 16,
+                                                 n_blk * BLOCK_N, n_valid, 1.0f, p);
+      }
     }
   }
 }
 
-template <int BLOCK_N, bool kBf16, int kEpi>
+template <int BLOCK_N, bool kBf16, int kEpi, bool kEpiWarps>
 __global__ void __launch_bounds__(kNumThreads, 1)
 gemm_tn_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
                const GemmParams p) {
-  gemm_body<BLOCK_N, kBf16, kEpi>(&tmap_a, &tmap_b, p);
+  gemm_body<BLOCK_N, kBf16, kEpi, kEpiWarps>(&tmap_a, &tmap_b, p);
 }
 
 // Same body with a tile width chosen at run time among 96..256 so that the tile count fills whole waves of SMs
 // (the M = 4680/N-row shards of the multi-GPU mode).
-template <int BLOCK_N, bool kBf16, int kEpi>
+template <int BLOCK_N, bool kBf16, int kEpi, bool kEpiWarps>
 __global__ void __launch_bounds__(kNumThreads, 1)
 gemm_flex_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
                  const GemmParams p) {
-  gemm_body<BLOCK_N, kBf16, kEpi>(&tmap_a, &tmap_b, p);
+  gemm_body<BLOCK_N, kBf16, kEpi, kEpiWarps>(&tmap_a, &tmap_b, p);
 }
 
 // ---------------------------------------------------------------------------
 // host launcher
 // ---------------------------------------------------------------------------
+// KR_GEMM_EPI_WARPS: 1 = the 16-bit epilogues run on the epilogue warps (default), 0 = in the consumer registers
+static bool gemm_epi_warps() {
+  static const bool on = [] { const char* e = getenv("KR_GEMM_EPI_WARPS"); return e == nullptr || atoi(e) != 0; }();
+  return on;
+}
+
 template <int BLOCK_N, bool kBf16, int kEpi>
 static int launch_gemm(const void* a, int lda, const void* w, int ldw, const GemmParams& p,
                        cudaStream_t stream) {
-  using Cfg = GemmCfg<BLOCK_N>;
+  constexpr bool kSplit = kEpi != EPI_F32;
+  const bool split = kSplit && gemm_epi_warps();
   CUtensorMap ta, tb;
   int rc = make_tmap_2d(&ta, a, p.M, p.K, lda, BLOCK_M, BLOCK_K, kBf16);
   if (rc != KR_OK) return rc;
   rc = make_tmap_2d(&tb, w, p.N, p.K, ldw, BLOCK_N, BLOCK_K, kBf16);
   if (rc != KR_OK) return rc;
-  auto kern = gemm_tn_kernel<BLOCK_N, kBf16, kEpi>;
-  static bool attr_set = false;
+  auto kern = split ? gemm_tn_kernel<BLOCK_N, kBf16, kEpi, kSplit> : gemm_tn_kernel<BLOCK_N, kBf16, kEpi, false>;
+  const int smem_bytes = split ? GemmCfg<BLOCK_N, true>::kSmemBytes : GemmCfg<BLOCK_N, false>::kSmemBytes;
+  static bool attr_set = false;   // the switch is read once per process, so `kern` is fixed per instantiation
   if (!attr_set) {
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                         Cfg::kSmemBytes);
+                                         smem_bytes);
     if (e != cudaSuccess) {
       set_last_error("gemm: cudaFuncSetAttribute failed: %s", cudaGetErrorString(e));
       return KR_ERR_CUDA;
@@ -162,7 +330,7 @@ static int launch_gemm(const void* a, int lda, const void* w, int ldw, const Gem
   const int num_tiles = ((p.M + BLOCK_M - 1) / BLOCK_M) * ((p.N + BLOCK_N - 1) / BLOCK_N);
   int grid = sm_count();
   if (grid > num_tiles) grid = num_tiles;
-  kern<<<grid, kNumThreads, Cfg::kSmemBytes, stream>>>(ta, tb, p);
+  kern<<<grid, kNumThreads, smem_bytes, stream>>>(ta, tb, p);
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) {
     set_last_error("gemm: launch failed: %s", cudaGetErrorString(e));
@@ -207,16 +375,18 @@ int gemm_flex_bn(int epi, int M, int N, int K) {
 
 template <int BN, bool kBf16, int kEpi>
 static int launch_flex(const void* a, int lda, const void* w, int ldw, const GemmParams& p, cudaStream_t stream) {
-  using Cfg = GemmCfg<BN>;
+  static_assert(kEpi != EPI_F32, "the runtime-width kernel serves the 16-bit epilogues");
+  const bool split = gemm_epi_warps();
   CUtensorMap ta, tb;
   int rc = make_tmap_2d(&ta, a, p.M, p.K, lda, BLOCK_M, BLOCK_K, kBf16);
   if (rc != KR_OK) return rc;
   rc = make_tmap_2d(&tb, w, p.N, p.K, ldw, BN, BLOCK_K, kBf16);
   if (rc != KR_OK) return rc;
-  auto kern = gemm_flex_kernel<BN, kBf16, kEpi>;
-  static bool attr_set = false;
+  auto kern = split ? gemm_flex_kernel<BN, kBf16, kEpi, true> : gemm_flex_kernel<BN, kBf16, kEpi, false>;
+  const int smem_bytes = split ? GemmCfg<BN, true>::kSmemBytes : GemmCfg<BN, false>::kSmemBytes;
+  static bool attr_set = false;   // the switch is read once per process, so `kern` is fixed per instantiation
   if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes);
+    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes);
     if (e != cudaSuccess) {
       set_last_error("gemm_flex: cudaFuncSetAttribute failed: %s", cudaGetErrorString(e));
       return KR_ERR_CUDA;
@@ -226,7 +396,7 @@ static int launch_flex(const void* a, int lda, const void* w, int ldw, const Gem
   const int num_tiles = ((p.M + BLOCK_M - 1) / BLOCK_M) * ((p.N + BN - 1) / BN);
   int grid = sm_count();
   if (grid > num_tiles) grid = num_tiles;
-  kern<<<grid, kNumThreads, Cfg::kSmemBytes, stream>>>(ta, tb, p);
+  kern<<<grid, kNumThreads, smem_bytes, stream>>>(ta, tb, p);
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) {
     set_last_error("gemm_flex: launch failed: %s", cudaGetErrorString(e));
