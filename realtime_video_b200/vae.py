@@ -15,7 +15,9 @@ Cache semantics (reference vae.py:191-206, vae_block3.py:46-91):
     (sentinel, vae_block3.py:51-53); one-frame chunks then update the cache as
     [where(old_last == 0, 0, x), x] (vae_block3.py:56-60) — reproduced verbatim.
 Latent frames of one call are processed together per layer (one launch per conv), which is
-arithmetically identical to the reference's frame-by-frame loop because every conv is causal.
+arithmetically identical to the reference's frame-by-frame loop because every conv is causal.  For the same reason
+the high-resolution stages may run over a chunk one frame tile at a time when whole-chunk buffers would exceed the
+engine's memory budget (1280x720); the buffers there then hold [2 + tile] frames.
 """
 from __future__ import annotations
 
@@ -228,6 +230,23 @@ def _vae_attention(b, x):
     return out
 
 
+GiB = 1 << 30
+
+
+def _buf_bytes(plan) -> int:
+    """Bytes of the conv-input buffers of a plan [(conv, shape, dtype)]."""
+    return sum(math.prod(shape) * dt.itemsize for _, shape, dt in plan)
+
+
+def _pick_frame_tile(frames: int, nbytes, untiled_max: int, tiled_max: int) -> int:
+    """Frames per tile of an engine's high-resolution stages.  Buffers for the whole chunk (``frames``) give the fewest
+    and fullest launches and are kept while ``nbytes(frames) <= untiled_max``; otherwise the largest tile whose
+    buffers fit ``tiled_max`` (at least one frame).  Each extra tile costs one 2-frame cache roll per conv."""
+    if nbytes(frames) <= untiled_max:
+        return frames
+    return max((t for t in range(1, frames) if nbytes(t) <= tiled_max), default=1)
+
+
 class _CacheList(list):
     """The feature-cache list handed to the caller: a plain ``list`` that can be weakly referenced."""
     __slots__ = ("__weakref__",)
@@ -286,10 +305,15 @@ class DecoderEngine(_StreamLedger):
     """Runs VAEDecoder3d (+ the wrapper's un-scale and conv2) on the sm_90a kernels."""
 
     MAX_CHUNK = 3          # latent frames per launch sequence
+    # Conv-input buffer budget.  832x480 keeps whole-chunk buffers (11.0 GiB, beside the 480p session); 1280x720
+    # (25.4 GiB untiled) runs the stages after the last up3d time step in frame tiles to stay within 8 GiB.
+    UNTILED_MAX_BYTES = 12 * GiB
+    TILED_MAX_BYTES = 8 * GiB
 
     def __init__(self, decoder: VAEDecoder3d, conv2: nn.Module, mean: torch.Tensor, std: torch.Tensor,
                  single_mode: bool = False, quant: Optional[str] = None):
         self.decoder, self.conv2, self.mean, self.std = decoder, conv2, mean, std
+        self._tile_override: Optional[int] = None     # frames per tile instead of the budget's choice (tests)
         # None: fp16 / bf16 everywhere; "fp8": residual.2 / residual.6 of every ResidualBlock and head.2 run on e4m3
         # inputs and weights (fp16 only).  Part of the prepared-weights key: switching rebuilds the buffers.
         self.quant = quant
@@ -304,7 +328,7 @@ class DecoderEngine(_StreamLedger):
             raise ValueError(f"VAE decoder quant must be 'fp8' or None, got {self.quant!r}")
         if self.quant == "fp8" and dtype != torch.float16:
             raise ValueError(f"the FP8 VAE tier runs in float16, got {dtype}")
-        key = (dtype, str(device), H, W, _weights_tag(self.decoder.conv1.weight), self.quant)
+        key = (dtype, str(device), H, W, _weights_tag(self.decoder.conv1.weight), self.quant, self._tile_override)
         if self._key == key:
             return
         d = self.decoder
@@ -346,31 +370,50 @@ class DecoderEngine(_StreamLedger):
                     _to_fp8(b["c1"], b["g1"])
                     _to_fp8(b["c2"], b["g2"])
             _to_fp8(self.head, self.g_head)
+        # the frame-tiled segment: the spatial half of the last up3d and everything after it
+        self._split = max(i for i, b in enumerate(self.blocks) if b["kind"] == "up" and b["mode"] == "upsample3d")
         self._key = key
         self._alloc(H, W)
 
-    def _alloc(self, H, W):
-        """Persistent conv-input buffers (cache frames in front) for a chunk of MAX_CHUNK latent
-        frames; spatial size doubles at every Resample, frames double at every up3d."""
-        dt, dev = self.dtype, self.device
-        T = self.MAX_CHUNK
+    def _buf_plan(self, H, W, tile):
+        """[(conv, buffer shape, dtype)]: conv-input buffers (cache frames in front) for a chunk of MAX_CHUNK latent
+        frames; spatial size doubles at every Resample, frames double at every up3d, and the tiled segment holds
+        ``tile`` frames."""
+        plan = []
 
         def buf(conv: _Conv, t, h, w):
-            conv.buf = torch.zeros(conv.taps[0] - 1 + t, h, w, conv.cin, device=dev,
-                                   dtype=torch.float8_e4m3fn if conv.in_scale is not None else dt)
+            plan.append((conv, (conv.taps[0] - 1 + t, h, w, conv.cin),
+                         torch.float8_e4m3fn if conv.in_scale is not None else self.dtype))
 
-        buf(self.conv1, T, H, W)
-        h, w, t = H, W, T
-        for b in self.blocks:
+        t = self.MAX_CHUNK
+        buf(self.conv1, t, H, W)
+        h, w = H, W
+        for i, b in enumerate(self.blocks):
             if b["kind"] == "res":
                 buf(b["c1"], t, h, w)
                 buf(b["c2"], t, h, w)
             elif b["kind"] == "up":
                 if b["mode"] == "upsample3d":
-                    b["tcache"] = torch.zeros(2, h, w, b["C"], dtype=dt, device=dev)
                     t *= 2
+                if i == self._split:
+                    t = min(t, tile)
                 h, w = 2 * h, 2 * w
         buf(self.head, t, h, w)
+        return plan
+
+    def _alloc(self, H, W):
+        dt, dev = self.dtype, self.device
+        frames = self.MAX_CHUNK << sum(b["kind"] == "up" and b["mode"] == "upsample3d" for b in self.blocks)
+        self.frame_tile = self._tile_override or _pick_frame_tile(
+            frames, lambda t: _buf_bytes(self._buf_plan(H, W, t)), self.UNTILED_MAX_BYTES, self.TILED_MAX_BYTES)
+        for conv, shape, bdt in self._buf_plan(H, W, self.frame_tile):
+            conv.buf = torch.zeros(shape, dtype=bdt, device=dev)
+        h, w = H, W
+        for b in self.blocks:
+            if b["kind"] == "up":
+                if b["mode"] == "upsample3d":
+                    b["tcache"] = torch.zeros(2, h, w, b["C"], dtype=dt, device=dev)
+                h, w = 2 * h, 2 * w
         self.initialised = False       # no frame decoded yet (first-frame sentinel state)
 
     def reset(self):
@@ -442,89 +485,114 @@ class DecoderEngine(_StreamLedger):
         assert T <= self.MAX_CHUNK and (not first or T == 1)
         c1 = self.conv1
         ops.vae_scale_input(z, self.mean_d, self.inv_std_d, self.w2, self.b2, c1.buf[2:2 + T])
-        blocks = self.blocks
         h, w = self.H, self.W
-
-        def next_gamma(i):
-            """gamma of the norm that consumes block i's output (next ResidualBlock / head)."""
-            if i + 1 < len(blocks):
-                nb = blocks[i + 1]
-                return (nb["g1"], nb["c1"]) if nb["kind"] == "res" else (None, None)
-            return self.g_head, self.head
 
         # conv1 -> raw x (residual stream) + normalised input of middle.0.conv1
         x = self._new(T, h, w, c1.cout)
-        g, nxt = blocks[0]["g1"], blocks[0]["c1"]
+        g, nxt = self.blocks[0]["g1"], self.blocks[0]["c1"]
         self._conv(c1, T, out_raw=x, out_norm=nxt.buf[2:2 + T], gamma=g, norm_scale=nxt.in_scale)
 
-        for i, b in enumerate(blocks):
-            if b["kind"] == "res":
-                ca, cb = b["c1"], b["c2"]
-                res = x
-                if b["sc"] is not None:
-                    res = self._new(T, h, w, b["cout"])
-                    self._conv(b["sc"], T, src=x, out_raw=res)
-                self._conv(ca, T, out_norm=cb.buf[2:2 + T], gamma=b["g2"], norm_scale=cb.in_scale)
-                g, nxt = next_gamma(i)
-                need_raw = nxt is not self.head          # the head only needs the normalised tensor
-                xo = self._new(T, h, w, b["cout"]) if need_raw else None
-                self._conv(cb, T, residual=res, out_raw=xo,
-                           out_norm=nxt.buf[2:2 + T] if g is not None else None, gamma=g,
-                           norm_scale=nxt.in_scale if g is not None else None)
-                x = xo
-            elif b["kind"] == "attn":
-                x = self._attention(b, x)
-                nb = blocks[i + 1]
-                if nb["c1"].in_scale is not None:
-                    ops.vae_rmsnorm_silu_fp8(x, nb["g1"], nb["c1"].buf[2:2 + T], nb["c1"].in_scale)
-                else:
-                    ops.vae_rmsnorm_silu(x, nb["g1"], nb["c1"].buf[2:2 + T])
-            else:  # Resample
-                C = b["C"]
-                if b["mode"] == "upsample3d":
-                    if first and self.single_mode:
-                        # demo_utils/vae.py:112-123: [zeros, x] on the channel axis -> after the
-                        # channel->time interleave a ZERO frame precedes every frame; cache untouched
-                        y = torch.zeros(2 * T, h, w, C, dtype=self.dtype, device=self.device)
-                        y[1::2] = x
-                        x, T = y, 2 * T
-                    elif first:
-                        b["tcache"].zero_()                    # sentinel, time_conv skipped
-                    else:
-                        tc = b["tconv"]
-                        y = self._new(2 * T, h, w, C)
-                        frame = h * w * C
-                        # chunk-wise cache update of vae_block3.py:55-62 per reference chunk
-                        step = self._chunk_frames(i)
-                        for s0 in range(0, T, step):
-                            xin = torch.cat([b["tcache"], x[s0:s0 + step]], dim=0)
-                            for half in range(2):
-                                ops.vae_conv(xin, tc.weight[half * C:(half + 1) * C], tc.bias[half * C:],
-                                             n=C, cout=C, T=step, taps=tc.taps, tile=_tile_for(h, w),
-                                             out_raw=y[2 * s0 + half:], raw_frame_stride=2 * frame)
-                            xs = x[s0:s0 + step]
-                            if step >= 2:
-                                b["tcache"].copy_(xs[-2:])
-                            elif self.single_mode:         # demo_utils/vae.py:106-111: [0, x]
-                                b["tcache"][0].zero_()
-                                b["tcache"][1].copy_(xs[0])
-                            else:
-                                old_last = b["tcache"][1]
-                                pad = torch.where(old_last == 0, torch.zeros_like(xs[0]), xs[0])
-                                b["tcache"][0].copy_(pad)
-                                b["tcache"][1].copy_(xs[0])
-                        x, T = y, 2 * T
-                up = ops.vae_upsample2x(x, self._new(T, 2 * h, 2 * w, C))
-                h, w = 2 * h, 2 * w
-                cv = b["conv"]
-                x = self._new(T, h, w, cv.cout)
-                g, nxt = next_gamma(i)
-                self._conv(cv, T, src=up, out_raw=x, out_norm=nxt.buf[2:2 + T], gamma=g, norm_scale=nxt.in_scale)
-        # head conv -> clamped fp32 pixels [T, 3, H, W]
-        pix = torch.empty(T, 3, h, w, dtype=torch.float32, device=self.device)
-        self._conv(self.head, T, out_pix=pix)
+        s = self._split
+        for i in range(s):
+            x, T, h, w = self._block(i, x, T, h, w, first)
+        x, T = self._up_time(s, x, T, h, w, first)
+        # the high-resolution segment tile by tile: every conv in it is causal and carries its own 2-frame history, so
+        # a frame tile gives the same result as the whole chunk
+        pix = torch.empty(T, 3, 8 * self.H, 8 * self.W, dtype=torch.float32, device=self.device)
+        for f0 in range(0, T, self.frame_tile):
+            t = min(self.frame_tile, T - f0)
+            xt, ht, wt = self._up_space(s, x[f0:f0 + t], t, h, w)
+            for i in range(s + 1, len(self.blocks)):
+                xt, t, ht, wt = self._block(i, xt, t, ht, wt, first)
+            self._conv(self.head, t, out_pix=pix[f0:f0 + t])          # head conv -> clamped fp32 pixels
         self.initialised = True
         return pix
+
+    def _next_norm(self, i):
+        """gamma and conv of the norm that consumes block i's output (next ResidualBlock / head)."""
+        if i + 1 < len(self.blocks):
+            nb = self.blocks[i + 1]
+            return (nb["g1"], nb["c1"]) if nb["kind"] == "res" else (None, None)
+        return self.g_head, self.head
+
+    def _block(self, i, x, T, h, w, first):
+        """Block i on the frames x [T, h, w, C] -> (x, T, h, w) of its output."""
+        b = self.blocks[i]
+        if b["kind"] == "res":
+            ca, cb = b["c1"], b["c2"]
+            res = x
+            if b["sc"] is not None:
+                res = self._new(T, h, w, b["cout"])
+                self._conv(b["sc"], T, src=x, out_raw=res)
+            self._conv(ca, T, out_norm=cb.buf[2:2 + T], gamma=b["g2"], norm_scale=cb.in_scale)
+            g, nxt = self._next_norm(i)
+            need_raw = nxt is not self.head          # the head only needs the normalised tensor
+            xo = self._new(T, h, w, b["cout"]) if need_raw else None
+            self._conv(cb, T, residual=res, out_raw=xo,
+                       out_norm=nxt.buf[2:2 + T] if g is not None else None, gamma=g,
+                       norm_scale=nxt.in_scale if g is not None else None)
+            return xo, T, h, w
+        if b["kind"] == "attn":
+            x = self._attention(b, x)
+            nb = self.blocks[i + 1]
+            if nb["c1"].in_scale is not None:
+                ops.vae_rmsnorm_silu_fp8(x, nb["g1"], nb["c1"].buf[2:2 + T], nb["c1"].in_scale)
+            else:
+                ops.vae_rmsnorm_silu(x, nb["g1"], nb["c1"].buf[2:2 + T])
+            return x, T, h, w
+        x, T = self._up_time(i, x, T, h, w, first)
+        x, h, w = self._up_space(i, x, T, h, w)
+        return x, T, h, w
+
+    def _up_time(self, i, x, T, h, w, first):
+        """Time step of Resample i: the up3d time_conv doubles the frames (identity for up2d) -> (x, T)."""
+        b = self.blocks[i]
+        if b["mode"] != "upsample3d":
+            return x, T
+        C = b["C"]
+        if first and self.single_mode:
+            # demo_utils/vae.py:112-123: [zeros, x] on the channel axis -> after the
+            # channel->time interleave a ZERO frame precedes every frame; cache untouched
+            y = torch.zeros(2 * T, h, w, C, dtype=self.dtype, device=self.device)
+            y[1::2] = x
+            return y, 2 * T
+        if first:
+            b["tcache"].zero_()                    # sentinel, time_conv skipped
+            return x, T
+        tc = b["tconv"]
+        y = self._new(2 * T, h, w, C)
+        frame = h * w * C
+        # chunk-wise cache update of vae_block3.py:55-62 per reference chunk
+        step = self._chunk_frames(i)
+        for s0 in range(0, T, step):
+            xin = torch.cat([b["tcache"], x[s0:s0 + step]], dim=0)
+            for half in range(2):
+                ops.vae_conv(xin, tc.weight[half * C:(half + 1) * C], tc.bias[half * C:],
+                             n=C, cout=C, T=step, taps=tc.taps, tile=_tile_for(h, w),
+                             out_raw=y[2 * s0 + half:], raw_frame_stride=2 * frame)
+            xs = x[s0:s0 + step]
+            if step >= 2:
+                b["tcache"].copy_(xs[-2:])
+            elif self.single_mode:         # demo_utils/vae.py:106-111: [0, x]
+                b["tcache"][0].zero_()
+                b["tcache"][1].copy_(xs[0])
+            else:
+                old_last = b["tcache"][1]
+                pad = torch.where(old_last == 0, torch.zeros_like(xs[0]), xs[0])
+                b["tcache"][0].copy_(pad)
+                b["tcache"][1].copy_(xs[0])
+        return y, 2 * T
+
+    def _up_space(self, i, x, T, h, w):
+        """Spatial step of Resample i: nearest 2x upsample and its 3x3 conv -> (x, 2h, 2w)."""
+        b = self.blocks[i]
+        up = ops.vae_upsample2x(x, self._new(T, 2 * h, 2 * w, b["C"]))
+        h, w = 2 * h, 2 * w
+        cv = b["conv"]
+        x = self._new(T, h, w, cv.cout)
+        g, nxt = self._next_norm(i)
+        self._conv(cv, T, src=up, out_raw=x, out_norm=nxt.buf[2:2 + T], gamma=g, norm_scale=nxt.in_scale)
+        return x, h, w
 
     def _chunk_frames(self, block_index: int) -> int:
         """Frames per REFERENCE chunk (one latent frame) at the input of Resample `block_index`:
@@ -731,15 +799,19 @@ class EncoderEngine(_StreamLedger):
     causal conv owns a persistent input buffer whose two leading frames ARE its feature cache."""
 
     MAX_CHUNK = 4          # pixel frames per later chunk
+    # Conv-input buffer budget: 832x480 keeps 4-frame buffers (3.1 GiB); 1280x720 (7.2 GiB untiled) runs the full- and
+    # half-resolution stages in frame tiles.
+    UNTILED_MAX_BYTES = TILED_MAX_BYTES = 4.5 * GiB
 
     def __init__(self, encoder: Encoder3d, conv1: nn.Module, mean: torch.Tensor, std: torch.Tensor):
         self.encoder, self.conv1_mod, self.mean, self.std = encoder, conv1, mean, std
+        self._tile_override: Optional[int] = None     # frames per tile instead of the budget's choice (tests)
         self._key = None
         self.initialised = False
 
     def _prepare(self, dtype, device, H, W):
         e = self.encoder
-        key = (dtype, str(device), H, W, _weights_tag(e.conv1.weight))
+        key = (dtype, str(device), H, W, _weights_tag(e.conv1.weight), self._tile_override)
         if self._key == key:
             return
         pc = lambda m, **kw: _prep_conv(m.weight.data, m.bias.data, dtype, device, **kw)  # noqa: E731
@@ -772,22 +844,45 @@ class EncoderEngine(_StreamLedger):
         self.b_out = self.conv1_mod.bias.data.to(device=device, dtype=dtype).contiguous()
         self.mean_d = self.mean.to(device=device, dtype=dtype)
         self.inv_std_d = 1.0 / self.std.to(device=device, dtype=dtype)
-        # conv-input buffers [2 history frames + up to t frames]; t halves at every downsample3d
-        z = lambda t, h, w, c: torch.zeros(2 + t, h, w, c, dtype=dtype, device=device)  # noqa: E731
-        t = self.MAX_CHUNK
-        self.conv_in.buf = z(t, H, W, 64)
+        # the frame-tiled segment: conv_in up to the first downsample3d's time_conv
+        self._split = next(i for i, b in enumerate(self.blocks) if b["kind"] == "down" and b["mode"] == "downsample3d")
+        self.frame_tile = self._tile_override or _pick_frame_tile(
+            self.MAX_CHUNK, lambda t: _buf_bytes(self._buf_plan(H, W, t)), self.UNTILED_MAX_BYTES,
+            self.TILED_MAX_BYTES)
+        for conv, shape, bdt in self._buf_plan(H, W, self.frame_tile):
+            conv.buf = torch.zeros(shape, dtype=bdt, device=device)
         h, w = H, W
         for b in self.blocks:
-            if b["kind"] == "res":
-                b["c1"].buf, b["c2"].buf = z(t, h, w, b["cin"]), z(t, h, w, b["cout"])
-            elif b["kind"] == "down":
+            if b["kind"] == "down":
                 h, w = h // 2, w // 2
                 if b["mode"] == "downsample3d":
                     b["tcache"] = torch.zeros(1, h, w, b["C"], dtype=dtype, device=device)
-                    t = max(1, t // 2)
-        self.head.buf = z(t, h, w, self.head.cin)
         self._key = key
         self.initialised = False
+
+    def _buf_plan(self, H, W, tile):
+        """[(conv, buffer shape, dtype)]: conv-input buffers [2 history frames + up to t frames]; t is the frame tile
+        in the tiled segment, then MAX_CHUNK halved at every downsample3d."""
+        plan = []
+
+        def buf(conv: _Conv, t, h, w):
+            plan.append((conv, (2 + t, h, w, conv.cin), self.dtype))
+
+        t = min(tile, self.MAX_CHUNK)
+        buf(self.conv_in, t, H, W)
+        h, w = H, W
+        for i, b in enumerate(self.blocks):
+            if b["kind"] == "res":
+                buf(b["c1"], t, h, w)
+                buf(b["c2"], t, h, w)
+            elif b["kind"] == "down":
+                h, w = h // 2, w // 2
+                if i == self._split:
+                    t = self.MAX_CHUNK
+                if b["mode"] == "downsample3d":
+                    t = max(1, t // 2)
+        buf(self.head, t, h, w)
+        return plan
 
     # -- stream state ------------------------------------------------------------------------------
     def _cache_tensors(self):
@@ -833,70 +928,103 @@ class EncoderEngine(_StreamLedger):
     def encode_chunk(self, frames: torch.Tensor, first: bool) -> torch.Tensor:
         """frames [T, 3, H, W] in [-1, 1] (T == 1 when ``first``, else 4) -> mu [16, T', H/8, W/8] with
         T' = 1: the scaled latent frame of this chunk."""
-        dt, dev = self.dtype, self.device
         T = frames.shape[0]
         assert (T == 1) if first else (T == self.MAX_CHUNK), "chunks are 1 frame (first) or 4 frames"
-        new = lambda t, h, w, c: torch.empty(t, h, w, c, dtype=dt, device=dev)  # noqa: E731
-        cin = self.conv_in
-        cin.buf[2:2 + T, :, :, :3] = frames.to(dt).permute(0, 2, 3, 1)
-        blocks = self.blocks
-
-        def next_norm(i):
-            if i + 1 < len(blocks):
-                nb = blocks[i + 1]
-                return (nb["g1"], nb["c1"]) if nb["kind"] == "res" else (None, None)
-            return self.g_head, self.head
-
-        h, w = self.H, self.W
-        x = new(T, h, w, cin.cout)
-        self._conv(cin, T, out_raw=x, out_norm=blocks[0]["c1"].buf[2:2 + T], gamma=blocks[0]["g1"])
-        for i, b in enumerate(blocks):
-            if b["kind"] == "res":
-                res = x
-                if b["sc"] is not None:
-                    res = new(T, h, w, b["cout"])
-                    self._conv(b["sc"], T, src=x, out_raw=res)
-                self._conv(b["c1"], T, out_norm=b["c2"].buf[2:2 + T], gamma=b["g2"])
-                g, nxt = next_norm(i)
-                need_raw = nxt is not self.head
-                xo = new(T, h, w, b["cout"]) if need_raw else None
-                self._conv(b["c2"], T, residual=res, out_raw=xo,
-                           out_norm=nxt.buf[2:2 + T] if g is not None else None, gamma=g)
-                x = xo
-            elif b["kind"] == "attn":
-                x = _vae_attention(b, x)
-                nb = blocks[i + 1]
-                ops.vae_rmsnorm_silu(x, nb["g1"], nb["c1"].buf[2:2 + T])
-            else:   # Resample: stride-2 conv behind ZeroPad2d((0,1,0,1)) per frame (vae.py:84-92, :152-155)
-                g, nxt = next_norm(i)
-                C = b["C"]
-                h, w = h // 2, w // 2
-                if b["mode"] != "downsample3d" or first:
-                    xo = new(T, h, w, C)
-                    self._conv(b["conv"], T, src=x, out_raw=xo, out_norm=nxt.buf[2:2 + T], gamma=g, sub2=True)
-                    if b["mode"] == "downsample3d":
-                        b["tcache"].copy_(xo)                 # first chunk: remember, skip time_conv (:160-163)
-                    x = xo
-                else:
-                    # [last cached frame, T frames] -> time_conv (3,1,1), stride 2 in time: T/2 frames (:164-171)
-                    xin = new(T + 1, h, w, C)
-                    xin[:1].copy_(b["tcache"])
-                    self._conv(b["conv"], T, src=x, out_raw=xin[1:], sub2=True)
-                    b["tcache"].copy_(xin[T:T + 1])
-                    tc = b["tconv"]
-                    T2 = T // 2
-                    xo = new(T2, h, w, C)
-                    for j in range(T2):
-                        ops.vae_conv(xin[2 * j:2 * j + 3], tc.weight, tc.bias, n=tc.n, cout=tc.cout, T=1, taps=tc.taps,
-                                     tile=_tile_for(h, w), out_raw=xo[j:j + 1], out_norm=nxt.buf[2 + j:3 + j], gamma=g)
-                    x, T = xo, T2
-        y = new(T, h, w, self.head.cout)
+        cin, blocks, s = self.conv_in, self.blocks, self._split
+        # the high-resolution segment tile by tile (every conv in it is causal and carries its own 2-frame history);
+        # its last stride-2 conv writes the frames the first downsample3d's time_conv reads, after one cached frame
+        xin = None
+        for f0 in range(0, T, self.frame_tile):
+            t = min(self.frame_tile, T - f0)
+            h, w = self.H, self.W
+            cin.buf[2:2 + t, :, :, :3] = frames[f0:f0 + t].to(self.dtype).permute(0, 2, 3, 1)
+            x = self._new(t, h, w, cin.cout)
+            self._conv(cin, t, out_raw=x, out_norm=blocks[0]["c1"].buf[2:2 + t], gamma=blocks[0]["g1"])
+            for i in range(s):
+                x, t, h, w = self._block(i, x, t, h, w, first)
+            h, w = h // 2, w // 2
+            if xin is None:
+                xin = self._new(T + 1, h, w, blocks[s]["C"])
+            self._down_space(s, x, t, xin[1:], f0, first)
+        x, T = self._down_time(s, xin, T, first)
+        for i in range(s + 1, len(blocks)):
+            x, T, h, w = self._block(i, x, T, h, w, first)
+        y = self._new(T, h, w, self.head.cout)
         self._conv(self.head, T, out_raw=y)
         out = ops.gemm(y.view(T * h * w, self.head.cout), self.w_out, self.b_out)       # WanVAE_.conv1 (1x1x1)
         mu = out[:, :16]
         mu = (mu - self.mean_d.view(1, 16)) * self.inv_std_d.view(1, 16)               # vae_block3.py:168-172
         self.initialised = True
         return mu.reshape(T, h, w, 16).permute(3, 0, 1, 2)
+
+    def _new(self, t, h, w, c):
+        return torch.empty(t, h, w, c, dtype=self.dtype, device=self.device)
+
+    def _next_norm(self, i):
+        if i + 1 < len(self.blocks):
+            nb = self.blocks[i + 1]
+            return (nb["g1"], nb["c1"]) if nb["kind"] == "res" else (None, None)
+        return self.g_head, self.head
+
+    def _block(self, i, x, T, h, w, first):
+        """Block i on the frames x [T, h, w, C] -> (x, T, h, w) of its output."""
+        b = self.blocks[i]
+        if b["kind"] == "res":
+            res = x
+            if b["sc"] is not None:
+                res = self._new(T, h, w, b["cout"])
+                self._conv(b["sc"], T, src=x, out_raw=res)
+            self._conv(b["c1"], T, out_norm=b["c2"].buf[2:2 + T], gamma=b["g2"])
+            g, nxt = self._next_norm(i)
+            need_raw = nxt is not self.head
+            xo = self._new(T, h, w, b["cout"]) if need_raw else None
+            self._conv(b["c2"], T, residual=res, out_raw=xo,
+                       out_norm=nxt.buf[2:2 + T] if g is not None else None, gamma=g)
+            return xo, T, h, w
+        if b["kind"] == "attn":
+            x = _vae_attention(b, x)
+            nb = self.blocks[i + 1]
+            ops.vae_rmsnorm_silu(x, nb["g1"], nb["c1"].buf[2:2 + T])
+            return x, T, h, w
+        h, w = h // 2, w // 2
+        if b["mode"] != "downsample3d":
+            xo = self._new(T, h, w, b["C"])
+            self._down_space(i, x, T, xo, 0, first)
+            return xo, T, h, w
+        xin = self._new(T + 1, h, w, b["C"])
+        self._down_space(i, x, T, xin[1:], 0, first)
+        x, T = self._down_time(i, xin, T, first)
+        return x, T, h, w
+
+    def _down_space(self, i, x, T, out, f0, first):
+        """Resample i's stride-2 conv behind ZeroPad2d((0,1,0,1)) per frame (vae.py:84-92, :152-155) of frames
+        [f0, f0 + T) of the chunk into out[f0:]; it also writes the next norm's input unless a time_conv follows."""
+        b = self.blocks[i]
+        if b["mode"] != "downsample3d" or first:
+            g, nxt = self._next_norm(i)
+            self._conv(b["conv"], T, src=x, out_raw=out[f0:f0 + T], out_norm=nxt.buf[2 + f0:2 + f0 + T], gamma=g,
+                       sub2=True)
+        else:
+            self._conv(b["conv"], T, src=x, out_raw=out[f0:f0 + T], sub2=True)
+
+    def _down_time(self, i, xin, T, first):
+        """Time step of downsample3d i on xin [1 + T, h, w, C] (frames 1.. from _down_space) -> (x, T)."""
+        b = self.blocks[i]
+        if first:
+            b["tcache"].copy_(xin[T:T + 1])
+            return xin[1:], T                    # first chunk: remember, skip time_conv (:160-163)
+        # [last cached frame, T frames] -> time_conv (3,1,1), stride 2 in time: T/2 frames (:164-171)
+        xin[:1].copy_(b["tcache"])
+        b["tcache"].copy_(xin[T:T + 1])
+        g, nxt = self._next_norm(i)
+        h, w, C = xin.shape[1:]
+        tc = b["tconv"]
+        T2 = T // 2
+        xo = self._new(T2, h, w, C)
+        for j in range(T2):
+            ops.vae_conv(xin[2 * j:2 * j + 3], tc.weight, tc.bias, n=tc.n, cout=tc.cout, T=1, taps=tc.taps,
+                         tile=_tile_for(h, w), out_raw=xo[j:j + 1], out_norm=nxt.buf[2 + j:3 + j], gamma=g)
+        return xo, T2
 
     def encode_first(self, frame: torch.Tensor) -> torch.Tensor:
         """frame [3, H, W] -> mu [16, H/8, W/8] on a fresh stream (the server's first-frame re-encode)."""
