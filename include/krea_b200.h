@@ -108,6 +108,21 @@ int kr_gemm_fp8_rowwise(int epilogue, const void* a, int lda, const void* w, int
                         const void* residual, int ldr, const void* gate, int gate_stride, int rows_per_gate, void* out2,
                         int ldc2, int n_split, int row_offset, void* stream);
 
+/* Fast accumulation = torchao Float8MMConfig(use_fast_accum=True), i.e. torch._scaled_mm(use_fast_accum=True): the
+ * e4m3 tensor-core instruction accumulates in place across the whole K instead of being promoted to fp32 registers
+ * every 128 k.  Same arguments, operands and epilogues as kr_gemm_fp8 / kr_gemm_fp8_rowwise (the quantised bytes and
+ * scales do not depend on the mode); a 128 x 256 tile, so N % 256 == 0, K % 16 == 0, lda / ldw % 16 == 0, ldc % 8 == 0,
+ * else KR_ERR_INVALID_ARG.  The accumulator keeps fewer mantissa bits than fp32: see DESIGN.md section 5 for the
+ * measured difference. */
+int kr_gemm_fp8_fast(int epilogue, const void* a, int lda, const void* w, int ldw, const float* scale_a,
+                     float scale_w, const void* bias, void* out, int ldc, int M, int N, int K, const void* residual,
+                     int ldr, const void* gate, int gate_stride, int rows_per_gate, void* out2, int ldc2, int n_split,
+                     int row_offset, void* stream);
+int kr_gemm_fp8_rowwise_fast(int epilogue, const void* a, int lda, const void* w, int ldw, const float* scale_a,
+                             const float* scale_w, const void* bias, void* out, int ldc, int M, int N, int K,
+                             const void* residual, int ldr, const void* gate, int gate_stride, int rows_per_gate,
+                             void* out2, int ldc2, int n_split, int row_offset, void* stream);
+
 /* Which kernel kr_gemm launches for this epilogue and shape: 1 = the single-CTA kernel, 2 = the 2-CTA
  * cluster kernel (128x256 tile per CTA, W multicast to both), 3 = the stream-K kernel (only with a workspace), 4 = the
  * single-CTA kernel with a runtime tile width fitted to whole waves of SMs (small-M shards).  Host-only

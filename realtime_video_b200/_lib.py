@@ -129,10 +129,14 @@ SIGNATURES = {
                 _i, _vp],
     "kr_fp8_quantize": [_vp, _i, _i, _i, _vp, _i, _vp, _vp],
     "kr_gemm_fp8": [_i, _vp, _i, _vp, _i, _vp, _f, _vp, _vp, _i, _i, _i, _i, _vp, _i, _vp, _i, _i, _vp, _i, _i, _i, _vp],
+    "kr_gemm_fp8_fast": [_i, _vp, _i, _vp, _i, _vp, _f, _vp, _vp, _i, _i, _i, _i, _vp, _i, _vp, _i, _i, _vp, _i, _i, _i,
+                         _vp],
     "kr_fp8_quantize_rows": [_vp, _i, _i, _i, _vp, _i, _vp, _vp],
     "kr_ln_modulate_fp8": [_vp, _i, _vp, _i, _i, _i, _f, _vp, _vp, _vp, _i, _i, _i, _i, _i, _vp, _i, _vp, _vp],
     "kr_gemm_fp8_rowwise": [_i, _vp, _i, _vp, _i, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp, _i, _vp, _i, _i, _vp, _i,
                             _i, _i, _vp],
+    "kr_gemm_fp8_rowwise_fast": [_i, _vp, _i, _vp, _i, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp, _i, _vp, _i, _i, _vp,
+                                 _i, _i, _i, _vp],
     "kr_attn_fwd": [_i, _vp, _i, _vp, _i, _vp, _i, _vp, _i, _i, _i, _i, _f, _i, _i, _i, _i, _vp],
     "kr_t5_attn": [_vp, _i, _vp, _i, _vp, _i, _vp, _i, _i, _i, _vp, _vp, _vp],
     "kr_ln_modulate": [_vp, _i, _vp, _i, _i, _i, _f, _vp, _vp, _vp, _i, _i, _i, _i, _i, _vp],

@@ -106,6 +106,48 @@ int kr_gemm_fp8_rowwise(int epilogue, const void* a, int lda, const void* w, int
   return kr::gemm_fp8_rowwise_tn(epilogue, a, lda, w, ldw, p, scale_a, scale_w, static_cast<cudaStream_t>(stream));
 }
 
+// The fast-accumulation kernels tile N by 256; shapes they cannot run are argument errors, reported here so that a
+// caller (and a build without the kernels) sees them before anything touches the device.
+#define KR_REQUIRE_FP8_FAST_SHAPE()                                                              \
+  do {                                                                                           \
+    KR_REQUIRE(M > 0 && N > 0 && K > 0 && N % 256 == 0 && K % 16 == 0, "need N % 256 == 0 and K % 16 == 0"); \
+    KR_REQUIRE(lda % 16 == 0 && ldw % 16 == 0 && lda >= K && ldw >= K && ldc % 8 == 0 && ldc > 0,           \
+               "pitches: lda / ldw >= K and % 16 == 0, ldc % 8 == 0");                                     \
+  } while (0)
+
+int kr_gemm_fp8_fast(int epilogue, const void* a, int lda, const void* w, int ldw, const float* scale_a,
+                     float scale_w, const void* bias, void* out, int ldc, int M, int N, int K, const void* residual,
+                     int ldr, const void* gate, int gate_stride, int rows_per_gate, void* out2, int ldc2, int n_split,
+                     int row_offset, void* stream) {
+  KR_REQUIRE(a && w && out, "null a/w/out");
+  KR_REQUIRE(scale_a, "null scale_a");
+  KR_REQUIRE_FP8_FAST_SHAPE();
+  KR_REQUIRE_LINKED(gemm_fp8_fast_tn);
+  kr::GemmParams p;
+  p.out = out; p.bias = bias; p.residual = residual; p.gate = gate;
+  p.M = M; p.N = N; p.K = K; p.ldc = ldc; p.ldr = ldr; p.gate_stride = gate_stride;
+  p.rows_per_gate = rows_per_gate; p.alpha = 1.0f;
+  p.out2 = out2; p.ldc2 = ldc2; p.n_split = n_split; p.row_offset = row_offset;
+  return kr::gemm_fp8_fast_tn(epilogue, a, lda, w, ldw, p, scale_a, scale_w, static_cast<cudaStream_t>(stream));
+}
+
+int kr_gemm_fp8_rowwise_fast(int epilogue, const void* a, int lda, const void* w, int ldw, const float* scale_a,
+                             const float* scale_w, const void* bias, void* out, int ldc, int M, int N, int K,
+                             const void* residual, int ldr, const void* gate, int gate_stride, int rows_per_gate,
+                             void* out2, int ldc2, int n_split, int row_offset, void* stream) {
+  KR_REQUIRE(a && w && out, "null a/w/out");
+  KR_REQUIRE(scale_a && scale_w, "null scale_a/scale_w");
+  KR_REQUIRE_FP8_FAST_SHAPE();
+  KR_REQUIRE_LINKED(gemm_fp8_rowwise_fast_tn);
+  kr::GemmParams p;
+  p.out = out; p.bias = bias; p.residual = residual; p.gate = gate;
+  p.M = M; p.N = N; p.K = K; p.ldc = ldc; p.ldr = ldr; p.gate_stride = gate_stride;
+  p.rows_per_gate = rows_per_gate; p.alpha = 1.0f;
+  p.out2 = out2; p.ldc2 = ldc2; p.n_split = n_split; p.row_offset = row_offset;
+  return kr::gemm_fp8_rowwise_fast_tn(epilogue, a, lda, w, ldw, p, scale_a, scale_w,
+                                      static_cast<cudaStream_t>(stream));
+}
+
 int kr_attn_fwd(int dtype, const void* q, int ldq, const void* k, int ldk, const void* v, int ldv,
                 void* out, int ldo, int Lq, int Lkv, int heads, float softmax_scale, int mask_mode,
                 int block_len, int window, int pad_keys, void* stream) {

@@ -132,12 +132,14 @@ KR_DEVICE void release_stage(uint64_t* empty) {
 // Consumer side of the TMA ring for k-blocks [kb0, kb1) of one tile: the warpgroup multiplies its 64-row slice
 // (`a_base` already offset to it) of each stage's A tile with the stage's BN-row W tile.  One wgmma group stays in
 // flight; a stage is released (one arrive per warpgroup on `empty`) once the group reading it has retired.
-template <int BN, int kKind, int kCluster = 1>
+// kPromote (e4m3's default) instead retires every k-block into a scratch partial and adds it to `acc` in fp32;
+// e4m3 with kPromote = false accumulates in place like the 16-bit kinds (torch._scaled_mm's use_fast_accum).
+template <int BN, int kKind, int kCluster = 1, bool kPromote = (kKind == 2)>
 KR_DEVICE void gemm_mainloop(float (&acc)[BN / 2], uint32_t a_base, uint32_t b_base, int a_bytes, int b_bytes,
                              int stages, uint64_t* full, uint64_t* empty, int& stage, uint32_t& phase, int kb0,
                              int kb1) {
   const bool leader = (threadIdx.x & 127) == 0;
-  if constexpr (kKind == 2) {
+  if constexpr (kPromote) {
     // e4m3 wgmma accumulates with a reduced-precision adder: each k-block's partial product is added to the fp32
     // accumulator in registers (one wgmma group per k-block, retired before the add)
     float part[BN / 2];

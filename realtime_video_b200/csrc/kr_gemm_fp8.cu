@@ -16,8 +16,14 @@
 //
 // Kernel structure = kr_gemm.cu (persistent 1 CTA/SM, two consumer warpgroups with register accumulators, a TMA
 // warpgroup), with byte-sized elements: a 128-byte swizzle row holds 128 k-elements, one wgmma consumes K = 32
-// (32 bytes); each 128-wide k-block is accumulated separately and added to the fp32 registers (the e4m3 wgmma
-// adder keeps fewer mantissa bits), so the tile is 128 x 128 to leave registers for the partial.
+// (32 bytes).  Two kernels of that structure differ in how they accumulate:
+//   gemm_fp8_kernel      (promoted, the default): each 128-wide k-block is accumulated separately and added to the
+//                        fp32 registers (the e4m3 wgmma adder keeps fewer mantissa bits), so the tile is 128 x 128
+//                        to leave registers for the partial;
+//   gemm_fp8_fast_kernel (torchao Float8MMConfig(use_fast_accum=True) = torch._scaled_mm(use_fast_accum=True)): the
+//                        wgmma accumulates in place across the whole K with one group in flight, like the 16-bit
+//                        GEMM, so the registers hold a 128 x 256 tile (m64n256k32, half the shared-memory operand
+//                        bytes per FLOP) and the tensor cores are not drained after every k-block.
 #include "kr_common.cuh"
 #include "kr_gemm_epi.cuh"
 #include "kr_ops.h"
@@ -110,6 +116,89 @@ gemm_fp8_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constan
   }
 }
 
+// Fast accumulation: the body of gemm_fp8_kernel on a 128 x 256 tile, with gemm_mainloop accumulating in place (one
+// wgmma group in flight, a stage released when the group that read it has retired).  A kernel of its own rather than
+// a shared body: the promoted kernel must keep its machine code bit for bit, and routing it through a common
+// function changed its register allocation.
+namespace {
+constexpr int F8F_BN = 256, F8F_B_BYTES = F8F_BN * F8_BK, F8F_STAGE_BYTES = F8_A_BYTES + F8F_B_BYTES;
+constexpr int F8F_SMEM = F8_STAGES * F8F_STAGE_BYTES + F8_SCR_BYTES + 1024 + 256;
+static_assert(F8F_SMEM <= 227 * 1024, "4 stages of 16 KB A + 32 KB W and the epilogue scratch fit one SM");
+}  // namespace
+
+template <int kEpi, bool kRowwise>
+__global__ void __launch_bounds__(F8_THREADS, 1)
+gemm_fp8_fast_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
+                     const GemmParams p, const float* __restrict__ scale_a,
+                     const typename Fp8ScaleW<kRowwise>::type scale_w) {
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
+                                             ~static_cast<uintptr_t>(1023));
+  uint8_t* smem_a = smem;
+  uint8_t* smem_b = smem + F8_STAGES * F8_A_BYTES;
+  float* scratch = reinterpret_cast<float*>(smem + F8_STAGES * F8F_STAGE_BYTES);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + F8_STAGES * F8F_STAGE_BYTES + F8_SCR_BYTES);
+  uint64_t* full_bar = bars;
+  uint64_t* empty_bar = bars + F8_STAGES;
+
+  const int warp = threadIdx.x >> 5;
+  const int num_m = (p.M + F8_BM - 1) / F8_BM, num_n = p.N / F8F_BN, num_tiles = num_m * num_n;
+  const int num_k = (p.K + F8_BK - 1) / F8_BK;
+
+  if (threadIdx.x == 256) {
+    prefetch_tmap(&tmap_a);
+    prefetch_tmap(&tmap_b);
+    for (int i = 0; i < F8_STAGES; ++i) {
+      mbar_init(&full_bar[i], 1);
+      mbar_init(&empty_bar[i], 2);
+    }
+    fence_barrier_init();
+  }
+  __syncthreads();
+
+  if (warp >= 8) {
+    producer_regs();
+    if (warp == 8 && elect_one()) {
+      int stage = 0;
+      uint32_t phase = 0;
+      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+        const int m_blk = tile % num_m, n_blk = tile / num_m;
+        for (int kb = 0; kb < num_k; ++kb) {
+          mbar_wait(&empty_bar[stage], phase ^ 1);
+          mbar_expect_tx(&full_bar[stage], F8F_STAGE_BYTES);
+          tma_load_2d(smem_a + stage * F8_A_BYTES, &tmap_a, &full_bar[stage], kb * F8_BK, m_blk * F8_BM);
+          tma_load_2d(smem_b + stage * F8F_B_BYTES, &tmap_b, &full_bar[stage], kb * F8_BK, n_blk * F8F_BN);
+          if (++stage == F8_STAGES) {
+            stage = 0;
+            phase ^= 1;
+          }
+        }
+      }
+    }
+    return;
+  }
+  consumer_regs();
+  const int wg = warp >> 2;
+  const uint32_t a_base = smem_u32(smem_a) + wg * 64 * F8_BK, b_base = smem_u32(smem_b);
+  float* scr = scratch + warp * kEpiScrFloats;
+  float s = 1.f;
+  if constexpr (!kRowwise) s = __ldg(scale_a) * scale_w;
+  int stage = 0;
+  uint32_t phase = 0;
+  for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+    const int m_blk = tile % num_m, n_blk = tile / num_m;
+    float acc[F8F_BN / 2];
+    gemm_mainloop<F8F_BN, 2, 1, false>(acc, a_base, b_base, F8_A_BYTES, F8F_B_BYTES, F8_STAGES, full_bar, empty_bar,
+                                       stage, phase, 0, num_k);
+    if constexpr (kRowwise)
+      gemm_frag_epilogue<F8F_BN, true, kEpi, true>(acc, scr, m_blk * F8_BM + wg * 64 + (warp & 3) * 16, n_blk * F8F_BN,
+                                                   F8F_BN, s, p, scale_a, scale_w);
+    else
+      gemm_frag_epilogue<F8F_BN, true, kEpi>(acc, scr, m_blk * F8_BM + wg * 64 + (warp & 3) * 16, n_blk * F8F_BN,
+                                             F8F_BN, s, p);
+  }
+}
+
 // ---------------------------------------------------------------------------
 // dynamic per-tensor activation quantisation: amax -> scale -> saturating e4m3 cast
 // ---------------------------------------------------------------------------
@@ -187,9 +276,10 @@ int fp8_quantize(const void* x, long ld, int rows, int cols, void* q, long ldq, 
 // ---------------------------------------------------------------------------
 // host launcher
 // ---------------------------------------------------------------------------
-template <int kEpi, bool kRowwise>
+template <bool kFast, int kEpi, bool kRowwise>
 static int launch_fp8(const void* a, int lda, const void* w, int ldw, const GemmParams& p, const float* scale_a,
                       typename Fp8ScaleW<kRowwise>::type scale_w, cudaStream_t stream) {
+  constexpr int BN = kFast ? F8F_BN : F8_BN, SMEM = kFast ? F8F_SMEM : F8_SMEM;
   CUtensorMap ta, tb;
   // byte tensors: [rows, K] uint8, box [128 | 256 rows, 128 bytes], SWIZZLE_128B
   const uint64_t da[2] = {static_cast<uint64_t>(p.K), static_cast<uint64_t>(p.M)};
@@ -199,23 +289,23 @@ static int launch_fp8(const void* a, int lda, const void* w, int ldw, const Gemm
   if (rc != KR_OK) return rc;
   const uint64_t db[2] = {static_cast<uint64_t>(p.K), static_cast<uint64_t>(p.N)};
   const uint64_t sb[1] = {static_cast<uint64_t>(ldw)};
-  const uint32_t bb[2] = {F8_BK, F8_BN};
+  const uint32_t bb[2] = {F8_BK, BN};
   rc = make_tmap_u8(&tb, w, 2, db, sb, bb, 128);
   if (rc != KR_OK) return rc;
-  auto kern = gemm_fp8_kernel<kEpi, kRowwise>;
+  auto kern = kFast ? gemm_fp8_fast_kernel<kEpi, kRowwise> : gemm_fp8_kernel<kEpi, kRowwise>;
   static bool attr_set = false;
   if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, F8_SMEM);
+    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM);
     if (e != cudaSuccess) {
       set_last_error("gemm_fp8: cudaFuncSetAttribute failed: %s", cudaGetErrorString(e));
       return KR_ERR_CUDA;
     }
     attr_set = true;
   }
-  const int num_tiles = ((p.M + F8_BM - 1) / F8_BM) * (p.N / F8_BN);
+  const int num_tiles = ((p.M + F8_BM - 1) / F8_BM) * (p.N / BN);
   int grid = sm_count();
   if (grid > num_tiles) grid = num_tiles;
-  kern<<<grid, F8_THREADS, F8_SMEM, stream>>>(ta, tb, p, scale_a, scale_w);
+  kern<<<grid, F8_THREADS, SMEM, stream>>>(ta, tb, p, scale_a, scale_w);
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) {
     set_last_error("gemm_fp8: launch failed: %s", cudaGetErrorString(e));
@@ -224,10 +314,11 @@ static int launch_fp8(const void* a, int lda, const void* w, int ldw, const Gemm
   return KR_OK;
 }
 
-static int check_fp8(const char* who, int epi, int lda, int ldw, const GemmParams& p) {
-  if (p.M <= 0 || p.N <= 0 || p.K <= 0 || p.N % F8_BN != 0 || p.K % 16 != 0 || lda % 16 != 0 || ldw % 16 != 0 ||
+static int check_fp8(const char* who, int bn, int epi, int lda, int ldw, const GemmParams& p) {
+  if (p.M <= 0 || p.N <= 0 || p.K <= 0 || p.N % bn != 0 || p.K % 16 != 0 || lda % 16 != 0 || ldw % 16 != 0 ||
       p.ldc % 8 != 0) {
-    set_last_error("%s: unsupported shape M=%d N=%d K=%d (need N %% 128 == 0, K / ld %% 16 == 0)", who, p.M, p.N, p.K);
+    set_last_error("%s: unsupported shape M=%d N=%d K=%d (need N %% %d == 0, K / ld %% 16 == 0)", who, p.M, p.N, p.K,
+                   bn);
     return KR_ERR_UNSUPPORTED_SHAPE;
   }
   if ((epi == EPI_BIAS_GATE_RES || epi == EPI_BIAS_RES || epi == EPI_MUL) && p.residual == nullptr) {
@@ -237,42 +328,64 @@ static int check_fp8(const char* who, int epi, int lda, int ldw, const GemmParam
   return KR_OK;
 }
 
-int gemm_fp8_tn(int epi, const void* a, int lda, const void* w, int ldw, const GemmParams& p, const float* scale_a,
-                float scale_w, cudaStream_t stream) {
-  const int rc = check_fp8("gemm_fp8", epi, lda, ldw, p);
+template <bool kFast>
+static int gemm_fp8_any(const char* who, int epi, const void* a, int lda, const void* w, int ldw, const GemmParams& p,
+                        const float* scale_a, float scale_w, cudaStream_t stream) {
+  const int rc = check_fp8(who, kFast ? F8F_BN : F8_BN, epi, lda, ldw, p);
   if (rc != KR_OK) return rc;
   if (scale_a == nullptr) {
-    set_last_error("gemm_fp8: null activation scale");
+    set_last_error("%s: null activation scale", who);
     return KR_ERR_INVALID_ARG;
   }
   switch (epi) {
-    case EPI_BIAS: return launch_fp8<EPI_BIAS, false>(a, lda, w, ldw, p, scale_a, scale_w, stream);
-    case EPI_BIAS_GELU: return launch_fp8<EPI_BIAS_GELU, false>(a, lda, w, ldw, p, scale_a, scale_w, stream);
-    case EPI_BIAS_GATE_RES: return launch_fp8<EPI_BIAS_GATE_RES, false>(a, lda, w, ldw, p, scale_a, scale_w, stream);
-    case EPI_BIAS_RES: return launch_fp8<EPI_BIAS_RES, false>(a, lda, w, ldw, p, scale_a, scale_w, stream);
-    default: set_last_error("gemm_fp8: unsupported epilogue %d", epi); return KR_ERR_INVALID_ARG;
+    case EPI_BIAS: return launch_fp8<kFast, EPI_BIAS, false>(a, lda, w, ldw, p, scale_a, scale_w, stream);
+    case EPI_BIAS_GELU: return launch_fp8<kFast, EPI_BIAS_GELU, false>(a, lda, w, ldw, p, scale_a, scale_w, stream);
+    case EPI_BIAS_GATE_RES: return launch_fp8<kFast, EPI_BIAS_GATE_RES, false>(a, lda, w, ldw, p, scale_a, scale_w, stream);
+    case EPI_BIAS_RES: return launch_fp8<kFast, EPI_BIAS_RES, false>(a, lda, w, ldw, p, scale_a, scale_w, stream);
+    default: set_last_error("%s: unsupported epilogue %d", who, epi); return KR_ERR_INVALID_ARG;
   }
+}
+
+template <bool kFast>
+static int gemm_fp8_rowwise_any(const char* who, int epi, const void* a, int lda, const void* w, int ldw,
+                                const GemmParams& p, const float* scale_a, const float* scale_w, cudaStream_t stream) {
+  const int rc = check_fp8(who, kFast ? F8F_BN : F8_BN, epi, lda, ldw, p);
+  if (rc != KR_OK) return rc;
+  if (scale_a == nullptr || scale_w == nullptr) {
+    set_last_error("%s: null row or channel scales", who);
+    return KR_ERR_INVALID_ARG;
+  }
+  if (reinterpret_cast<uintptr_t>(scale_w) % 16 != 0) {
+    set_last_error("%s: channel scales must be 16-byte aligned", who);
+    return KR_ERR_INVALID_ARG;
+  }
+  switch (epi) {
+    case EPI_BIAS: return launch_fp8<kFast, EPI_BIAS, true>(a, lda, w, ldw, p, scale_a, scale_w, stream);
+    case EPI_BIAS_GELU: return launch_fp8<kFast, EPI_BIAS_GELU, true>(a, lda, w, ldw, p, scale_a, scale_w, stream);
+    case EPI_BIAS_GATE_RES: return launch_fp8<kFast, EPI_BIAS_GATE_RES, true>(a, lda, w, ldw, p, scale_a, scale_w, stream);
+    case EPI_BIAS_RES: return launch_fp8<kFast, EPI_BIAS_RES, true>(a, lda, w, ldw, p, scale_a, scale_w, stream);
+    default: set_last_error("%s: unsupported epilogue %d", who, epi); return KR_ERR_INVALID_ARG;
+  }
+}
+
+int gemm_fp8_tn(int epi, const void* a, int lda, const void* w, int ldw, const GemmParams& p, const float* scale_a,
+                float scale_w, cudaStream_t stream) {
+  return gemm_fp8_any<false>("gemm_fp8", epi, a, lda, w, ldw, p, scale_a, scale_w, stream);
 }
 
 int gemm_fp8_rowwise_tn(int epi, const void* a, int lda, const void* w, int ldw, const GemmParams& p,
                         const float* scale_a, const float* scale_w, cudaStream_t stream) {
-  const int rc = check_fp8("gemm_fp8_rowwise", epi, lda, ldw, p);
-  if (rc != KR_OK) return rc;
-  if (scale_a == nullptr || scale_w == nullptr) {
-    set_last_error("gemm_fp8_rowwise: null row or channel scales");
-    return KR_ERR_INVALID_ARG;
-  }
-  if (reinterpret_cast<uintptr_t>(scale_w) % 16 != 0) {
-    set_last_error("gemm_fp8_rowwise: channel scales must be 16-byte aligned");
-    return KR_ERR_INVALID_ARG;
-  }
-  switch (epi) {
-    case EPI_BIAS: return launch_fp8<EPI_BIAS, true>(a, lda, w, ldw, p, scale_a, scale_w, stream);
-    case EPI_BIAS_GELU: return launch_fp8<EPI_BIAS_GELU, true>(a, lda, w, ldw, p, scale_a, scale_w, stream);
-    case EPI_BIAS_GATE_RES: return launch_fp8<EPI_BIAS_GATE_RES, true>(a, lda, w, ldw, p, scale_a, scale_w, stream);
-    case EPI_BIAS_RES: return launch_fp8<EPI_BIAS_RES, true>(a, lda, w, ldw, p, scale_a, scale_w, stream);
-    default: set_last_error("gemm_fp8_rowwise: unsupported epilogue %d", epi); return KR_ERR_INVALID_ARG;
-  }
+  return gemm_fp8_rowwise_any<false>("gemm_fp8_rowwise", epi, a, lda, w, ldw, p, scale_a, scale_w, stream);
+}
+
+int gemm_fp8_fast_tn(int epi, const void* a, int lda, const void* w, int ldw, const GemmParams& p,
+                     const float* scale_a, float scale_w, cudaStream_t stream) {
+  return gemm_fp8_any<true>("gemm_fp8_fast", epi, a, lda, w, ldw, p, scale_a, scale_w, stream);
+}
+
+int gemm_fp8_rowwise_fast_tn(int epi, const void* a, int lda, const void* w, int ldw, const GemmParams& p,
+                             const float* scale_a, const float* scale_w, cudaStream_t stream) {
+  return gemm_fp8_rowwise_any<true>("gemm_fp8_rowwise_fast", epi, a, lda, w, ldw, p, scale_a, scale_w, stream);
 }
 
 }  // namespace kr

@@ -60,6 +60,14 @@ __attribute__((weak)) int ln_modulate_fp8(const void* x, int ldx, void* out, int
 __attribute__((weak)) int gemm_fp8_rowwise_tn(int epi, const void* a, int lda, const void* w, int ldw,
                                               const GemmParams& p, const float* scale_a, const float* scale_w,
                                               cudaStream_t stream);
+// The two FP8 GEMMs with fast accumulation (torchao Float8MMConfig(use_fast_accum=True)): in-place e4m3 wgmma
+// accumulation across the whole K on a 128 x 256 tile, kr_gemm_fp8.cu; N % 256 == 0.  Weak for the same reason.
+__attribute__((weak)) int gemm_fp8_fast_tn(int epi, const void* a, int lda, const void* w, int ldw,
+                                           const GemmParams& p, const float* scale_a, float scale_w,
+                                           cudaStream_t stream);
+__attribute__((weak)) int gemm_fp8_rowwise_fast_tn(int epi, const void* a, int lda, const void* w, int ldw,
+                                                   const GemmParams& p, const float* scale_a, const float* scale_w,
+                                                   cudaStream_t stream);
 // 2-CTA cluster variant (W multicast to both CTAs, 128x256 tile per CTA), kr_gemm2.cu; N % 256 == 0
 int gemm2_tn(int dtype, int epi, const void* a, int lda, const void* w, int ldw, const GemmParams& p,
              cudaStream_t stream);

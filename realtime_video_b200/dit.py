@@ -32,10 +32,13 @@ from . import fp8, ops
 def _linear(x, lin: nn.Linear, **kw) -> torch.Tensor:
     """nn.Linear of a DiT block on the GEMM kernels: bf16 by default, FP8 (dynamic activation cast + e4m3 wgmma GEMM)
     when ``realtime_video_b200.fp8.quantize_`` attached quantised weights to the module, with the granularity it
-    attached: per tensor, or per row (``x`` may then be an ``ops.Fp8Rows`` the LayerNorm already cast)."""
+    attached: per tensor, or per row (``x`` may then be an ``ops.Fp8Rows`` the LayerNorm already cast), and with the
+    accumulation mode it recorded (``fast_accum`` is passed only when chosen)."""
     q = getattr(lin, "_kr_fp8", None)
     if q is None:
         return ops.gemm(x, lin.weight, lin.bias, **kw)
+    if fp8.is_fast_accum(lin):
+        kw["fast_accum"] = True
     if fp8.is_rowwise(lin):
         return ops.linear_fp8_rowwise(x, q[0], q[1], lin.bias, **kw)
     return ops.linear_fp8(x, q[0], q[1], lin.bias, **kw)

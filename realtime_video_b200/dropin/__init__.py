@@ -15,6 +15,8 @@ resolving to the reference checkout, independent of the ``sys.path`` order:
     torchao.quantization.quant_api -> realtime_video_b200.fp8       (quantize_, Float8DynamicActivationFloat8WeightConfig,
                                                                      PerTensor: the `enable_fp8` lines release_server.py:179-182;
                                                                      PerRow: the same lines with granularity=PerRow() also resolve)
+    torchao.float8.inference   -> realtime_video_b200.fp8           (Float8MMConfig, where torchao defines it: the same lines
+                                                                     with mm_config=Float8MMConfig(use_fast_accum=True))
 
 The served module IS the product module (same object under both names), so ``isinstance`` checks and class
 identity hold across the two spellings.  The reference's ``CausalInferencePipeline`` and ``GenerationSession``
@@ -42,6 +44,8 @@ ALIASES = {
     # `enable_fp8: true` (release_server.py:179-182): quantize_ / Float8DynamicActivationFloat8WeightConfig / PerTensor
     # (or PerRow)
     "torchao.quantization.quant_api": "realtime_video_b200.fp8",
+    # Float8MMConfig, the mm_config argument of the config above, under the module torchao defines it in
+    "torchao.float8.inference": "realtime_video_b200.fp8",
 }
 
 

@@ -16,10 +16,23 @@ lines above work unchanged.
 depend on how the rows are split across GPUs.  The block schedule then runs ``kr_gemm_fp8_rowwise`` fed by
 ``kr_ln_modulate_fp8`` (the LayerNorm writes e4m3 bytes and row scales directly) or ``kr_fp8_quantize_rows``.
 
+``mm_config=Float8MMConfig(use_fast_accum=True)`` selects fast accumulation: the e4m3 wgmma accumulates in place across
+the whole K (``kr_gemm_fp8_fast`` / ``kr_gemm_fp8_rowwise_fast``, a 128 x 256 tile with MMAs kept in flight), which is
+what ``torch._scaled_mm(use_fast_accum=True)`` does and what torchao's config asks for when the caller passes no
+``mm_config`` (from torchao's published source; torchao is not in the image, so like the rest of the torchao parity
+this is unpinned).  This is the one place the default here differs from torchao's: ``mm_config=None`` keeps the
+promoted accumulation (every 128-wide k-block's partial sum is added to fp32 registers), because the tensor core's
+accumulator keeps fewer mantissa bits than fp32 and the promoted kernel is the one every earlier result was taken
+with.  ``KR_FP8_FAST_ACCUM=1`` in the environment makes ``quantize_`` calls that pass no ``mm_config`` choose fast
+accumulation, so the reference's unmodified lines reach it.  Weights and scales are the same bytes in both modes.
+
 Numerics are a separate tier from the bf16 headline: e4m3 has 3 mantissa bits; tests state the tolerance against the
 fp8 oracle (same quantisation, fp32 matmul) and against the bf16 path.
 """
 from __future__ import annotations
+
+import os
+from dataclasses import dataclass
 
 import torch
 from torch import nn
@@ -35,10 +48,34 @@ class PerRow:
     """Granularity marker (torchao.quantization.PerRow): per-row activation scales, per-output-channel weight scales."""
 
 
-class Float8DynamicActivationFloat8WeightConfig:
-    """``granularity``: ``PerTensor()`` or ``PerRow()``, alone or as an (activation, weight) pair of the same kind."""
+@dataclass(frozen=True)
+class Float8MMConfig:
+    """torchao.float8.inference.Float8MMConfig, field for field.  ``use_fast_accum=True`` runs the FP8 GEMM that
+    accumulates inside the tensor core across the whole K; ``False`` the one that promotes every 128-wide k-block to
+    fp32.  ``emulate`` and ``pad_inner_dim`` are not implemented (K % 16 == 0 holds for every DiT block linear)."""
+    emulate: bool = False
+    use_fast_accum: bool = False
+    pad_inner_dim: bool = False
 
-    def __init__(self, granularity=None, **unused):
+    def __post_init__(self):
+        if self.emulate or self.pad_inner_dim:
+            raise NotImplementedError("Float8MMConfig: emulate=True / pad_inner_dim=True are not implemented")
+
+
+def _fast_accum_default() -> bool:
+    """The A/B switch: ``KR_FP8_FAST_ACCUM=1`` makes quantize_ calls without an mm_config choose fast accumulation."""
+    return os.environ.get("KR_FP8_FAST_ACCUM", "0") not in ("", "0")
+
+
+class Float8DynamicActivationFloat8WeightConfig:
+    """``granularity``: ``PerTensor()`` or ``PerRow()``, alone or as an (activation, weight) pair of the same kind.
+    ``mm_config``: a :class:`Float8MMConfig`, or None for promoted accumulation (torchao's None means
+    ``use_fast_accum=True``; see the module docstring) unless ``KR_FP8_FAST_ACCUM=1``."""
+
+    def __init__(self, granularity=None, mm_config=None, **unused):
+        if mm_config is not None and not isinstance(mm_config, Float8MMConfig):
+            raise TypeError(f"mm_config must be a Float8MMConfig or None, got {type(mm_config).__name__}")
+        self.mm_config = mm_config
         g = PerTensor() if granularity is None else granularity
         if isinstance(g, (list, tuple)):
             if len(g) != 2:
@@ -75,16 +112,24 @@ def is_rowwise(lin: nn.Module) -> bool:
     return isinstance(getattr(lin, "_kr_fp8_granularity", None), PerRow)
 
 
+def is_fast_accum(lin: nn.Module) -> bool:
+    """True when :func:`quantize_` chose fast accumulation (``Float8MMConfig(use_fast_accum=True)``) for ``lin``."""
+    return getattr(lin, "_kr_fp8_fast_accum", False)
+
+
 @torch.no_grad()
 def quantize_(module: nn.Module, config=None, filter_fn=None) -> nn.Module:
     """In-place, like torchao's: every ``nn.Linear`` inside the DiT blocks of ``module`` (a WanDiffusionWrapper, a
     CausalWanModel or any container of CausalWanAttentionBlock) gets FP8 weights.  The bf16 weights stay in place
     (state_dict unchanged); call ``dequantize_`` to go back.  PerTensor attaches ``(w_q, scale_w float)``, PerRow
-    ``(w_q, scale_w fp32 [N])`` on the weight's device."""
+    ``(w_q, scale_w fp32 [N])`` on the weight's device.  The accumulation mode of ``config.mm_config`` is recorded
+    beside them; the weights and scales do not depend on it."""
     if config is not None and not isinstance(config, Float8DynamicActivationFloat8WeightConfig):
         raise NotImplementedError(f"unsupported quantisation config {type(config).__name__}")
     gran = config.granularity if config is not None else PerTensor()
     quant = quantize_weight_rows if isinstance(gran, PerRow) else quantize_weight
+    mm = config.mm_config if config is not None else None
+    fast = _fast_accum_default() if mm is None else mm.use_fast_accum
     from .dit import CausalWanAttentionBlock
     n = 0
     for blk in module.modules():
@@ -95,6 +140,10 @@ def quantize_(module: nn.Module, config=None, filter_fn=None) -> nn.Module:
                     (filter_fn is None or filter_fn(lin, name)):
                 lin._kr_fp8 = quant(lin.weight)
                 lin._kr_fp8_granularity = gran
+                if fast:
+                    lin._kr_fp8_fast_accum = True
+                elif hasattr(lin, "_kr_fp8_fast_accum"):
+                    del lin._kr_fp8_fast_accum
                 n += 1
     if n == 0:
         raise ValueError("quantize_: no DiT block linears found in the module")
@@ -105,6 +154,7 @@ def dequantize_(module: nn.Module) -> nn.Module:
     for lin in module.modules():
         if isinstance(lin, nn.Linear) and hasattr(lin, "_kr_fp8"):
             del lin._kr_fp8
-            if hasattr(lin, "_kr_fp8_granularity"):
-                del lin._kr_fp8_granularity
+            for attr in ("_kr_fp8_granularity", "_kr_fp8_fast_accum"):
+                if hasattr(lin, attr):
+                    delattr(lin, attr)
     return module

@@ -266,9 +266,11 @@ def fp8_quantize(x: torch.Tensor, q: Optional[torch.Tensor] = None, state: Optio
 def gemm_fp8(a_q: torch.Tensor, w_q: torch.Tensor, scale_a: torch.Tensor, scale_w: float,
              bias: Optional[torch.Tensor] = None, *, epilogue: int = EPI_BIAS, out: Optional[torch.Tensor] = None,
              residual: Optional[torch.Tensor] = None, gate: Optional[torch.Tensor] = None, rows_per_gate: int = 0,
-             out2: Optional[torch.Tensor] = None, n_split: int = 0, row_offset: int = 0) -> torch.Tensor:
+             out2: Optional[torch.Tensor] = None, n_split: int = 0, row_offset: int = 0,
+             fast_accum: bool = False) -> torch.Tensor:
     """out[M,N] (bf16) = epilogue((a_q[M,K] @ w_q[N,K]^T) * scale_a[1] * scale_w + bias); a_q / w_q e4m3 bytes,
-    scale_a the ``state`` tensor of :func:`fp8_quantize`."""
+    scale_a the ``state`` tensor of :func:`fp8_quantize`.  ``fast_accum`` runs kr_gemm_fp8_fast (accumulation inside
+    the tensor core across the whole K, torch._scaled_mm's ``use_fast_accum=True``) on the same operands."""
     _req(a_q, "a_q", torch.uint8); _req(w_q, "w_q", torch.uint8)
     M, K = a_q.shape
     N = w_q.shape[0]
@@ -279,11 +281,13 @@ def gemm_fp8(a_q: torch.Tensor, w_q: torch.Tensor, scale_a: torch.Tensor, scale_
     gs = gate.stride(0) if gate is not None and gate.dim() >= 2 else 0
     ldc2 = _rows2d(out2, "out2")[1] if out2 is not None else 0
     lib = _lib.load()
-    with _Timed("gemm_fp8", 2.0 * M * N * K):
-        rc = lib.kr_gemm_fp8(epilogue, a_q.data_ptr(), a_q.stride(0), w_q.data_ptr(), w_q.stride(0),
-                             scale_a.data_ptr() + 4, scale_w, _ptr(bias), out.data_ptr(), ldc, M, N, K, _ptr(residual),
-                             ldr, _ptr(gate), gs, rows_per_gate, _ptr(out2), ldc2, n_split, row_offset, _stream())
-    _lib.check(rc, "kr_gemm_fp8")
+    name = "kr_gemm_fp8_fast" if fast_accum else "kr_gemm_fp8"
+    with _Timed("gemm_fp8_fast" if fast_accum else "gemm_fp8", 2.0 * M * N * K):
+        rc = getattr(lib, name)(epilogue, a_q.data_ptr(), a_q.stride(0), w_q.data_ptr(), w_q.stride(0),
+                                scale_a.data_ptr() + 4, scale_w, _ptr(bias), out.data_ptr(), ldc, M, N, K,
+                                _ptr(residual), ldr, _ptr(gate), gs, rows_per_gate, _ptr(out2), ldc2, n_split,
+                                row_offset, _stream())
+    _lib.check(rc, name)
     _count()
     return out
 
@@ -377,9 +381,10 @@ def gemm_fp8_rowwise(a: Fp8Rows, w_q: torch.Tensor, scale_w: torch.Tensor, bias:
                      epilogue: int = EPI_BIAS, out: Optional[torch.Tensor] = None,
                      residual: Optional[torch.Tensor] = None, gate: Optional[torch.Tensor] = None,
                      rows_per_gate: int = 0, out2: Optional[torch.Tensor] = None, n_split: int = 0,
-                     row_offset: int = 0) -> torch.Tensor:
+                     row_offset: int = 0, fast_accum: bool = False) -> torch.Tensor:
     """out[M,N] (bf16) = epilogue((a.q[M,K] @ w_q[N,K]^T) * a.scale[m] * scale_w[n] + bias); w_q e4m3 bytes,
-    scale_w fp32 [N] (torch._scaled_mm with row-wise scales)."""
+    scale_w fp32 [N] (torch._scaled_mm with row-wise scales).  ``fast_accum`` runs kr_gemm_fp8_rowwise_fast
+    (``use_fast_accum=True``) on the same operands."""
     _req(a.q, "a.q", torch.uint8); _req(a.scale, "a.scale", torch.float32)
     _req(w_q, "w_q", torch.uint8); _req(scale_w, "scale_w", torch.float32)
     M, K = a.q.shape
@@ -394,12 +399,13 @@ def gemm_fp8_rowwise(a: Fp8Rows, w_q: torch.Tensor, scale_w: torch.Tensor, bias:
     gs = gate.stride(0) if gate is not None and gate.dim() >= 2 else 0
     ldc2 = _rows2d(out2, "out2")[1] if out2 is not None else 0
     lib = _lib.load()
-    with _Timed("gemm_fp8", 2.0 * M * N * K, sub="rowwise"):
-        rc = lib.kr_gemm_fp8_rowwise(epilogue, a.q.data_ptr(), a.q.stride(0), w_q.data_ptr(), w_q.stride(0),
-                                     a.scale.data_ptr(), scale_w.data_ptr(), _ptr(bias), out.data_ptr(), ldc, M, N, K,
-                                     _ptr(residual), ldr, _ptr(gate), gs, rows_per_gate, _ptr(out2), ldc2, n_split,
-                                     row_offset, _stream())
-    _lib.check(rc, "kr_gemm_fp8_rowwise")
+    name = "kr_gemm_fp8_rowwise_fast" if fast_accum else "kr_gemm_fp8_rowwise"
+    with _Timed("gemm_fp8_fast" if fast_accum else "gemm_fp8", 2.0 * M * N * K, sub="rowwise"):
+        rc = getattr(lib, name)(epilogue, a.q.data_ptr(), a.q.stride(0), w_q.data_ptr(), w_q.stride(0),
+                                a.scale.data_ptr(), scale_w.data_ptr(), _ptr(bias), out.data_ptr(), ldc, M, N, K,
+                                _ptr(residual), ldr, _ptr(gate), gs, rows_per_gate, _ptr(out2), ldc2, n_split,
+                                row_offset, _stream())
+    _lib.check(rc, name)
     _count()
     return out
 
