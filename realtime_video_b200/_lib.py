@@ -169,12 +169,13 @@ SAGE_SIGNATURES = {
     "kr_sage_attn": [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _f, _vp],
 }
 
-# the FP8 tier of the VAE decoder's convolutions (include/krea_b200_vae_fp8.h, kr_vae.cu); every function returns int
+# the FP8 tier of the VAE decoder's and encoder's convolutions (include/krea_b200_vae_fp8.h, kr_vae.cu); every function returns int
 VAE_FP8_SIGNATURES = {
     "kr_vae_conv_fp8": [_i, _i, _i, _vp, _i, _vp, _vp, _f, _i, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _vp, _l, _l,
                         _vp, _l, _l, _f, _vp, _vp, _l, _l, _vp, _vp],
     "kr_vae_rmsnorm_silu_fp8": [_vp, _vp, _vp, _l, _i, _f, _vp],
 }
+VAE_FP8_SIGNATURES["kr_vae_conv_fp8_sub2"] = VAE_FP8_SIGNATURES["kr_vae_conv_fp8"]
 
 
 def load() -> ctypes.CDLL:

@@ -174,11 +174,9 @@ KR_DEVICE void conv_epilogue_frag(const ConvParams& p, float (&acc)[N / 2 / kSpl
   }
 }
 
-template <int CIN, int N, bool kBf16, bool kNormF8 = false>
-__global__ void __launch_bounds__(kConvThreads, 1)
-conv_igemm_kernel(const __grid_constant__ CUtensorMap tm_in64, const __grid_constant__ CUtensorMap tm_in32,
-                  const __grid_constant__ CUtensorMap tm_w64, const __grid_constant__ CUtensorMap tm_w32,
-                  const ConvParams p) {
+template <int CIN, int N, bool kBf16, bool kNormF8>
+KR_DEVICE void conv_igemm_body(const CUtensorMap& tm_in64, const CUtensorMap& tm_in32, const CUtensorMap& tm_w64,
+                               const CUtensorMap& tm_w32, const ConvParams& p) {
   using Cfg = ConvCfg<CIN, N>;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
@@ -316,6 +314,24 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tm_in64, const __grid_cons
   }
 }
 
+template <int CIN, int N, bool kBf16, bool kNormF8 = false>
+__global__ void __launch_bounds__(kConvThreads, 1)
+conv_igemm_kernel(const __grid_constant__ CUtensorMap tm_in64, const __grid_constant__ CUtensorMap tm_in32,
+                  const __grid_constant__ CUtensorMap tm_w64, const __grid_constant__ CUtensorMap tm_w32,
+                  const ConvParams p) {
+  conv_igemm_body<CIN, N, kBf16, kNormF8>(tm_in64, tm_in32, tm_w64, tm_w32, p);
+}
+
+// The encoder tier's fp16 producers of e4m3 conv inputs that the fp16 path runs on this kernel (conv_in, the 384-channel
+// stride-2 conv, the (3,1,1) time_convs): the same kernel with an e4m3 out_norm, as entry points of their own.
+template <int CIN, int N>
+__global__ void __launch_bounds__(kConvThreads, 1)
+enc_igemm_conv_f8n_kernel(const __grid_constant__ CUtensorMap tm_in64, const __grid_constant__ CUtensorMap tm_in32,
+                          const __grid_constant__ CUtensorMap tm_w64, const __grid_constant__ CUtensorMap tm_w32,
+                          const ConvParams p) {
+  conv_igemm_body<CIN, N, false, true>(tm_in64, tm_in32, tm_w64, tm_w32, p);
+}
+
 // ---------------------------------------------------------------------------------------------
 // conv_halo_kernel: the 3x3-spatial convs of the wide stages (N = 96 / 192 output channels).
 //
@@ -349,148 +365,17 @@ struct HaloCfg {
 static constexpr int kHaloThreads = 384;
 
 
-template <int CIN, int N, bool kBf16, bool kNormF8 = false>
-__global__ void __launch_bounds__(kHaloThreads, 1)
-conv_halo_kernel(const __grid_constant__ CUtensorMap tm_in, const __grid_constant__ CUtensorMap tm_w,
-                 const ConvParams p) {
-  using Cfg = HaloCfg<CIN, N>;
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
-                                             ~static_cast<uintptr_t>(1023));
-  uint8_t* smem_a = smem;
-  uint8_t* smem_b = smem + Cfg::kAStages * Cfg::kABytes;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem_b + Cfg::kBStages * Cfg::kBBytes);
-  uint64_t* a_full = bars;                         // [kAStages]
-  uint64_t* a_empty = a_full + Cfg::kAStages;      // [kAStages]
-  uint64_t* b_full = a_empty + Cfg::kAStages;      // [kBStages]
-  uint64_t* b_empty = b_full + Cfg::kBStages;      // [kBStages]
+// conv_halo_kernel, and the same kernel under the name enc_halo_conv_f8n_kernel for the FP8 encoder tier's fp16
+// stride-2 convs with an e4m3 out_norm (96 and 192 channels).  Both names are generated from one definition.
+#define KR_CONV_HALO_KERNEL conv_halo_kernel
+#include "kr_vae_halo_kernel.cuh"
+#undef KR_CONV_HALO_KERNEL
+#define KR_CONV_HALO_KERNEL enc_halo_conv_f8n_kernel
+#include "kr_vae_halo_kernel.cuh"
+#undef KR_CONV_HALO_KERNEL
 
-  const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
-  const int items_w = (p.W + 15) / 16;
-  const int items_h = (p.H + 15) / 16;
-  const int items_per_frame = items_w * items_h;
-  const int num_items = p.T * items_per_frame;
-
-  if (threadIdx.x == 256) {
-    prefetch_tmap(&tm_in);
-    prefetch_tmap(&tm_w);
-    for (int i = 0; i < Cfg::kAStages; ++i) {
-      mbar_init(&a_full[i], 1);
-      mbar_init(&a_empty[i], 2);
-    }
-    for (int i = 0; i < Cfg::kBStages; ++i) {
-      mbar_init(&b_full[i], 1);
-      mbar_init(&b_empty[i], 2);
-    }
-    fence_barrier_init();
-  }
-  __syncthreads();
-
-  if (warp >= 8) {
-    // ===================== TMA producer =====================
-    producer_regs();
-    if (warp == 8 && elect_one()) {
-      int sa = 0, sb = 0;
-      uint32_t pa = 0, pb = 0;
-      for (int item = blockIdx.x; item < num_items; item += gridDim.x) {
-        const int t = item / items_per_frame;
-        const int rem = item % items_per_frame;
-        const int h0 = (rem / items_w) * 16;
-        const int w0 = (rem % items_w) * 16;
-        for (int kt = 0; kt < p.KT; ++kt) {
-          for (int c = 0; c < Cfg::kChunks; ++c) {
-            mbar_wait(&a_empty[sa], pa ^ 1);
-            mbar_expect_tx(&a_full[sa], Cfg::kABytes);
-            tma_load_4d(smem_a + sa * Cfg::kABytes, &tm_in, &a_full[sa], c * 64, w0 - 1, h0 - 1, t + kt);
-            if (++sa == Cfg::kAStages) {
-              sa = 0;
-              pa ^= 1;
-            }
-            for (int sp = 0; sp < 9; ++sp) {
-              mbar_wait(&b_empty[sb], pb ^ 1);
-              mbar_expect_tx(&b_full[sb], Cfg::kBBytes);
-              tma_load_2d(smem_b + sb * Cfg::kBBytes, &tm_w, &b_full[sb], (kt * 9 + sp) * CIN + c * 64, 0);
-              if (++sb == Cfg::kBStages) {
-                sb = 0;
-                pb ^= 1;
-              }
-            }
-          }
-        }
-      }
-    }
-    return;
-  }
-
-  // ===================== consumer warpgroup u: pixel tile u of the item =====================
-  consumer_regs();
-  const int u = warp >> 2;
-  const bool leader = (threadIdx.x & 127) == 0;
-  const uint32_t a0 = smem_u32(smem_a), b0 = smem_u32(smem_b);
-  int sa = 0, sb = 0;
-  uint32_t pa = 0, pb = 0;
-  for (int item = blockIdx.x; item < num_items; item += gridDim.x) {
-    float acc[2][N / 2];      // m64 halves: tile rows h 0..7 and 8..15
-    bool first = true;
-    for (int kt = 0; kt < p.KT; ++kt) {
-      for (int c = 0; c < Cfg::kChunks; ++c) {
-        const int ksteps = (c == Cfg::kChunks - 1) ? Cfg::kLastK : 4;
-        mbar_wait(&a_full[sa], pa);
-        const uint32_t a_st = a0 + sa * Cfg::kABytes;
-#pragma unroll 1
-        for (int sp = 0; sp < 9; ++sp) {
-          const int kh = sp / 3, kw = sp - kh * 3;
-          mbar_wait(&b_full[sb], pb);
-          const uint32_t b_st = b0 + sb * Cfg::kBBytes;
-          const uint32_t a_win = a_st + (kh * Cfg::kBoxW + 8 * u + kw) * 128;
-          wgmma_fence();
-#pragma unroll
-          for (int k = 0; k < 4; ++k) {
-            if (k < ksteps) {
-              const uint64_t bd = make_smem_desc(b_st + k * 32, 16, 1024);
-#pragma unroll
-              for (int mh = 0; mh < 2; ++mh) {
-                const uint64_t ad = make_smem_desc(a_win + mh * 8 * Cfg::kBoxW * 128 + k * 32, 16, Cfg::kBoxW * 128);
-                wgmma_ss<N, kBf16, 0>(acc[mh], ad, bd, (first && k == 0) ? 0 : 1);
-              }
-            }
-          }
-          wgmma_commit();
-          wgmma_wait<0>();
-          reg_fence(acc[0]);
-          reg_fence(acc[1]);
-          first = false;
-          if (leader) mbar_arrive(&b_empty[sb]);
-          if (++sb == Cfg::kBStages) {
-            sb = 0;
-            pb ^= 1;
-          }
-        }
-        if (leader) mbar_arrive(&a_empty[sa]);
-        if (++sa == Cfg::kAStages) {
-          sa = 0;
-          pa ^= 1;
-        }
-      }
-    }
-    const int t = item / items_per_frame;
-    const int rem = item % items_per_frame;
-#pragma unroll
-    for (int mh = 0; mh < 2; ++mh) {
-      int hh[2], ww[2];
-#pragma unroll
-      for (int r = 0; r < 2; ++r) {
-        const int px = mh * 64 + (warp & 3) * 16 + (lane >> 2) + 8 * r;   // pixel row of the 16 x 8 tile
-        hh[r] = (rem / items_w) * 16 + (px >> 3);
-        ww[r] = (rem % items_w) * 16 + u * 8 + (px & 7);
-      }
-      conv_epilogue_frag<N, kBf16, kNormF8>(p, acc[mh], t, hh, ww, lane);
-    }
-  }
-}
-
-template <int CIN, int N, bool kBf16, bool kNormF8 = false>
+// kEnc: the encoder tier's entry point (fp16 with an e4m3 out_norm)
+template <int CIN, int N, bool kBf16, bool kNormF8 = false, bool kEnc = false>
 static int launch_conv_halo(const void* in, int t_in, const void* wgt, int w_rows, const ConvParams& p,
                             cudaStream_t stream) {
   using Cfg = HaloCfg<CIN, N>;
@@ -508,7 +393,13 @@ static int launch_conv_halo(const void* in, int t_in, const void* wgt, int w_row
   const uint32_t wbox[2] = {64, static_cast<uint32_t>(N)};
   rc = make_tmap_nd(&tw, wgt, 2, wdims, wstr, wbox, kBf16, 128);
   if (rc != KR_OK) return rc;
-  auto kern = conv_halo_kernel<CIN, N, kBf16, kNormF8>;
+  void (*kern)(const CUtensorMap, const CUtensorMap, const ConvParams);
+  if constexpr (kEnc) {
+    static_assert(kNormF8 && !kBf16, "encoder producers write e4m3 from fp16");
+    kern = enc_halo_conv_f8n_kernel<CIN, N, false, true>;
+  } else {
+    kern = conv_halo_kernel<CIN, N, kBf16, kNormF8>;
+  }
   static bool attr_set = false;
   if (!attr_set) {
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes);
@@ -533,7 +424,7 @@ static int launch_conv_halo(const void* in, int t_in, const void* wgt, int w_row
 // ---------------------------------------------------------------------------
 // host launcher
 // ---------------------------------------------------------------------------
-template <int CIN, int N, bool kBf16, bool kNormF8 = false>
+template <int CIN, int N, bool kBf16, bool kNormF8 = false, bool kEnc = false>
 static int launch_conv(const void* in, int t_in, const void* wgt, int w_rows, const ConvParams& p,
                        cudaStream_t stream) {
   using Cfg = ConvCfg<CIN, N>;
@@ -561,7 +452,13 @@ static int launch_conv(const void* in, int t_in, const void* wgt, int w_rows, co
     rc = make_tmap_nd(&w32, wgt, 2, wdims, wstr, wbox32, kBf16, 64);
     if (rc != KR_OK) return rc;
   }
-  auto kern = conv_igemm_kernel<CIN, N, kBf16, kNormF8>;
+  void (*kern)(const CUtensorMap, const CUtensorMap, const CUtensorMap, const CUtensorMap, const ConvParams);
+  if constexpr (kEnc) {
+    static_assert(kNormF8 && !kBf16, "encoder producers write e4m3 from fp16");
+    kern = enc_igemm_conv_f8n_kernel<CIN, N>;
+  } else {
+    kern = conv_igemm_kernel<CIN, N, kBf16, kNormF8>;
+  }
   static bool attr_set = false;
   if (!attr_set) {
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize,
@@ -698,9 +595,7 @@ struct HaloF8Cfg {
 };
 
 template <int CIN, int N>
-__global__ void __launch_bounds__(kHaloThreads, 1)
-conv_f8_halo_kernel(const __grid_constant__ CUtensorMap tm_in, const __grid_constant__ CUtensorMap tm_w,
-                    const ConvParams p) {
+KR_DEVICE void conv_f8_halo_body(const CUtensorMap& tm_in, const CUtensorMap& tm_w, const ConvParams p) {
   using Cfg = HaloF8Cfg<CIN, N>;
   using Ch = F8Chunks<CIN>;
   extern __shared__ uint8_t smem_raw[];
@@ -841,6 +736,21 @@ conv_f8_halo_kernel(const __grid_constant__ CUtensorMap tm_in, const __grid_cons
   }
 }
 
+template <int CIN, int N>
+__global__ void __launch_bounds__(kHaloThreads, 1)
+conv_f8_halo_kernel(const __grid_constant__ CUtensorMap tm_in, const __grid_constant__ CUtensorMap tm_w,
+                    const ConvParams p) {
+  conv_f8_halo_body<CIN, N>(tm_in, tm_w, p);
+}
+
+// The encoder tier's e4m3 halo conv of ResidualBlock(96, 192).residual.2, as an entry point of its own.
+template <int CIN, int N>
+__global__ void __launch_bounds__(kHaloThreads, 1)
+enc_f8_halo_conv_kernel(const __grid_constant__ CUtensorMap tm_in, const __grid_constant__ CUtensorMap tm_w,
+                        const ConvParams p) {
+  conv_f8_halo_body<CIN, N>(tm_in, tm_w, p);
+}
+
 // Per-tap variant (conv_igemm_kernel with byte elements and one 128-channel chunk per stage).  N = 384 does not fit
 // twice in a warpgroup's registers, so there the work unit is 64 pixels (one half of the TH x TW tile, box
 // {128, TW, TH/2}) and consumer warpgroup j owns channels [192 j, 192 j + 192) of it (96 accumulators + 96 partial);
@@ -861,9 +771,7 @@ struct ConvF8Cfg {
 };
 
 template <int CIN, int N>
-__global__ void __launch_bounds__(kConvThreads, 1)
-conv_f8_igemm_kernel(const __grid_constant__ CUtensorMap tm_in, const __grid_constant__ CUtensorMap tm_w,
-                     const ConvParams p) {
+KR_DEVICE void conv_f8_igemm_body(const CUtensorMap& tm_in, const CUtensorMap& tm_w, const ConvParams& p) {
   using Cfg = ConvF8Cfg<CIN, N>;
   using Ch = F8Chunks<CIN>;
   extern __shared__ uint8_t smem_raw[];
@@ -984,7 +892,23 @@ conv_f8_igemm_kernel(const __grid_constant__ CUtensorMap tm_in, const __grid_con
   }
 }
 
-template <int CIN, int N, bool kHalo>
+template <int CIN, int N>
+__global__ void __launch_bounds__(kConvThreads, 1)
+conv_f8_igemm_kernel(const __grid_constant__ CUtensorMap tm_in, const __grid_constant__ CUtensorMap tm_w,
+                     const ConvParams p) {
+  conv_f8_igemm_body<CIN, N>(tm_in, tm_w, p);
+}
+
+// The encoder tier's e4m3 head (384 -> 32 channels), as an entry point of its own.
+template <int CIN, int N>
+__global__ void __launch_bounds__(kConvThreads, 1)
+enc_f8_igemm_conv_kernel(const __grid_constant__ CUtensorMap tm_in, const __grid_constant__ CUtensorMap tm_w,
+                         const ConvParams p) {
+  conv_f8_igemm_body<CIN, N>(tm_in, tm_w, p);
+}
+
+// kEnc: the encoder tier's entry points
+template <int CIN, int N, bool kHalo, bool kEnc = false>
 static int launch_conv_f8(const void* in, int t_in, const void* wgt, int w_rows, const ConvParams& p,
                           cudaStream_t stream) {
   CUtensorMap tin, tw;
@@ -1002,14 +926,16 @@ static int launch_conv_f8(const void* in, int t_in, const void* wgt, int w_rows,
     using Cfg = HaloF8Cfg<CIN, N>;
     ibox[0] = 128; ibox[1] = Cfg::kBoxW; ibox[2] = Cfg::kBoxH; ibox[3] = 1;
     wbox[0] = 128; wbox[1] = N;
-    kern = conv_f8_halo_kernel<CIN, N>;
+    if constexpr (kEnc) kern = enc_f8_halo_conv_kernel<CIN, N>;
+    else kern = conv_f8_halo_kernel<CIN, N>;
     smem_bytes = Cfg::kSmemBytes;
     units = p.T * ((p.W + 15) / 16) * ((p.H + Cfg::kItemH - 1) / Cfg::kItemH);
   } else {
     using Cfg = ConvF8Cfg<CIN, N>;
     ibox[0] = 128; ibox[1] = p.TW; ibox[2] = p.TH / Cfg::kSplit; ibox[3] = 1;
     wbox[0] = 128; wbox[1] = Cfg::kWN;
-    kern = conv_f8_igemm_kernel<CIN, N>;
+    if constexpr (kEnc) kern = enc_f8_igemm_conv_kernel<CIN, N>;
+    else kern = conv_f8_igemm_kernel<CIN, N>;
     smem_bytes = Cfg::kSmemBytes;
     units = p.T * ((p.W + p.TW - 1) / p.TW) * ((p.H + p.TH - 1) / p.TH) * Cfg::kSplit;
   }
@@ -1038,7 +964,8 @@ static int launch_conv_f8(const void* in, int t_in, const void* wgt, int w_rows,
 }
 
 // in_fp8 = 1: e4m3 operands -> conv_f8_*; in_fp8 = 0: fp16 operands with an e4m3 out_norm (the producers of the FP8
-// convs' inputs that are not FP8 convs themselves: conv1 and the Resample convs)
+// convs' inputs that are not FP8 convs themselves: the decoder's conv1 and Resample convs, the encoder's conv_in,
+// stride-2 convs and time_convs).
 static int vae_conv_fp8(int in_fp8, int cin, int n, const void* in, int t_in, const void* wgt, int w_rows,
                         const ConvParams& p, cudaStream_t s) {
   const bool halo_taps = p.KH == 3 && p.KW == 3 && (p.KT == 1 || p.KT == 3) && w_rows >= n;
@@ -1048,10 +975,20 @@ static int vae_conv_fp8(int in_fp8, int cin, int n, const void* in, int t_in, co
     if (cin == 384 && n == 384) return launch_conv_f8<384, 384, false>(in, t_in, wgt, w_rows, p, s);
     if (cin == 192 && n == 384) return launch_conv_f8<192, 384, false>(in, t_in, wgt, w_rows, p, s);
     if (cin == 96 && n == 16) return launch_conv_f8<96, 16, false>(in, t_in, wgt, w_rows, p, s);
+    // encoder
+    if (halo_taps && cin == 96 && n == 192) return launch_conv_f8<96, 192, true, true>(in, t_in, wgt, w_rows, p, s);
+    if (cin == 384 && n == 32) return launch_conv_f8<384, 32, false, true>(in, t_in, wgt, w_rows, p, s);
   } else {
     if (halo_taps && cin == 384 && n == 192) return launch_conv_halo<384, 192, false, true>(in, t_in, wgt, w_rows, p, s);
     if (halo_taps && cin == 192 && n == 96) return launch_conv_halo<192, 96, false, true>(in, t_in, wgt, w_rows, p, s);
     if (cin == 64 && n == 384) return launch_conv<64, 384, false, true>(in, t_in, wgt, w_rows, p, s);
+    // encoder
+    if (halo_taps && cin == 96 && n == 96) return launch_conv_halo<96, 96, false, true, true>(in, t_in, wgt, w_rows, p, s);
+    if (halo_taps && cin == 192 && n == 192)
+      return launch_conv_halo<192, 192, false, true, true>(in, t_in, wgt, w_rows, p, s);
+    if (cin == 64 && n == 96) return launch_conv<64, 96, false, true, true>(in, t_in, wgt, w_rows, p, s);
+    if (cin == 192 && n == 192) return launch_conv<192, 192, false, true, true>(in, t_in, wgt, w_rows, p, s);
+    if (cin == 384 && n == 384) return launch_conv<384, 384, false, true, true>(in, t_in, wgt, w_rows, p, s);
   }
   set_last_error("vae_conv_fp8: unsupported configuration in_fp8=%d cin=%d n=%d taps=%dx%dx%d", in_fp8, cin, n, p.KT,
                  p.KH, p.KW);
@@ -1385,12 +1322,13 @@ int frames_to_rgb8(const float* pixels, uint8_t* rgb, int frames, int height, in
     }                                              \
   } while (0)
 
-extern "C" int kr_vae_conv_fp8(int in_fp8, int cin, int n, const void* in, int t_in, const void* weight,
-                               const float* w_scale, float in_scale, int w_rows, const void* bias, int cout, int T,
-                               int H, int W, int tile_w, int tile_h, int kt, int kh, int kw, void* out_raw,
-                               long raw_pix, long raw_frame, void* out_norm, long norm_pix, long norm_frame,
-                               float norm_q_scale, const void* gamma, const void* residual, long res_pix,
-                               long res_frame, float* out_pix, void* stream) {
+// kr_vae_conv_fp8 (sub2 = 0) and kr_vae_conv_fp8_sub2 (sub2 = 1)
+static int vae_conv_fp8_entry(int in_fp8, int cin, int n, const void* in, int t_in, const void* weight,
+                              const float* w_scale, float in_scale, int w_rows, const void* bias, int cout, int T,
+                              int H, int W, int tile_w, int tile_h, int kt, int kh, int kw, void* out_raw,
+                              long raw_pix, long raw_frame, void* out_norm, long norm_pix, long norm_frame,
+                              float norm_q_scale, const void* gamma, const void* residual, long res_pix,
+                              long res_frame, float* out_pix, int sub2, void* stream) {
   KR_VAE_F8_REQUIRE(in && weight, "null input/weight");
   KR_VAE_F8_REQUIRE(in_fp8 == 0 || in_fp8 == 1, "in_fp8 must be 0 or 1");
   KR_VAE_F8_REQUIRE(out_raw || out_norm || out_pix, "no output requested");
@@ -1403,6 +1341,8 @@ extern "C" int kr_vae_conv_fp8(int in_fp8, int cin, int n, const void* in, int t
   KR_VAE_F8_REQUIRE(tile_w * tile_h == 128 && T > 0 && H > 0 && W > 0, "bad geometry");
   KR_VAE_F8_REQUIRE((kt == 1 || kt == 3) && (kh == 1 || kh == 3) && (kw == 1 || kw == 3), "taps must be 1 or 3");
   KR_VAE_F8_REQUIRE(t_in >= T + kt - 1, "input holds too few frames");
+  KR_VAE_F8_REQUIRE(!sub2 || (!in_fp8 && out_pix == nullptr && kt == 1 && kh == 3 && kw == 3),
+                    "sub2 is the 16-bit 3x3 stride-2 conv");
   kr::ConvParams p;
   p.T = T; p.H = H; p.W = W; p.TW = tile_w; p.TH = tile_h; p.KT = kt; p.KH = kh; p.KW = kw;
   p.cout = cout;
@@ -1410,11 +1350,33 @@ extern "C" int kr_vae_conv_fp8(int in_fp8, int cin, int n, const void* in, int t
   p.out_norm = out_norm; p.norm_pix = norm_pix; p.norm_frame = norm_frame;
   p.out_pix = out_pix; p.bias = bias;
   p.residual = residual; p.res_pix = res_pix; p.res_frame = res_frame;
-  p.gamma = gamma; p.norm_scale = sqrtf(static_cast<float>(cout)); p.sub2 = 0;
+  p.gamma = gamma; p.norm_scale = sqrtf(static_cast<float>(cout)); p.sub2 = sub2;
   p.norm_q_scale = norm_q_scale;
   p.in_dequant = in_fp8 ? 1.0f / in_scale : 0.f;
   p.w_scale = w_scale;
   return kr::vae_conv_fp8(in_fp8, cin, n, in, t_in, weight, w_rows, p, static_cast<cudaStream_t>(stream));
+}
+
+extern "C" int kr_vae_conv_fp8(int in_fp8, int cin, int n, const void* in, int t_in, const void* weight,
+                               const float* w_scale, float in_scale, int w_rows, const void* bias, int cout, int T,
+                               int H, int W, int tile_w, int tile_h, int kt, int kh, int kw, void* out_raw,
+                               long raw_pix, long raw_frame, void* out_norm, long norm_pix, long norm_frame,
+                               float norm_q_scale, const void* gamma, const void* residual, long res_pix,
+                               long res_frame, float* out_pix, void* stream) {
+  return vae_conv_fp8_entry(in_fp8, cin, n, in, t_in, weight, w_scale, in_scale, w_rows, bias, cout, T, H, W, tile_w,
+                            tile_h, kt, kh, kw, out_raw, raw_pix, raw_frame, out_norm, norm_pix, norm_frame,
+                            norm_q_scale, gamma, residual, res_pix, res_frame, out_pix, 0, stream);
+}
+
+extern "C" int kr_vae_conv_fp8_sub2(int in_fp8, int cin, int n, const void* in, int t_in, const void* weight,
+                                    const float* w_scale, float in_scale, int w_rows, const void* bias, int cout,
+                                    int T, int H, int W, int tile_w, int tile_h, int kt, int kh, int kw,
+                                    void* out_raw, long raw_pix, long raw_frame, void* out_norm, long norm_pix,
+                                    long norm_frame, float norm_q_scale, const void* gamma, const void* residual,
+                                    long res_pix, long res_frame, float* out_pix, void* stream) {
+  return vae_conv_fp8_entry(in_fp8, cin, n, in, t_in, weight, w_scale, in_scale, w_rows, bias, cout, T, H, W, tile_w,
+                            tile_h, kt, kh, kw, out_raw, raw_pix, raw_frame, out_norm, norm_pix, norm_frame,
+                            norm_q_scale, gamma, residual, res_pix, res_frame, out_pix, 1, stream);
 }
 
 extern "C" int kr_vae_rmsnorm_silu_fp8(const void* x, void* y, const void* gamma, long pixels, int C, float q_scale,

@@ -681,8 +681,8 @@ def _(z, first, handle):
 # ---------------------------------------------------------------------------------------------
 # the reference-facing wrappers
 # ---------------------------------------------------------------------------------------------
-def _default_quant() -> Optional[str]:
-    return "fp8" if os.environ.get("KR_VAE_FP8", "0") not in ("", "0") else None
+def _default_quant(var: str = "KR_VAE_FP8") -> Optional[str]:
+    return "fp8" if os.environ.get(var, "0") not in ("", "0") else None
 
 
 class VAEDecoderWrapper(nn.Module):
@@ -799,19 +799,27 @@ class EncoderEngine(_StreamLedger):
     causal conv owns a persistent input buffer whose two leading frames ARE its feature cache."""
 
     MAX_CHUNK = 4          # pixel frames per later chunk
-    # Conv-input buffer budget: 832x480 keeps 4-frame buffers (3.1 GiB); 1280x720 (7.2 GiB untiled) runs the full- and
-    # half-resolution stages in frame tiles.
+    # Conv-input buffer budget: 832x480 keeps 4-frame buffers (3.1 GiB; 1.7 GiB on the FP8 tier); 1280x720 (7.2 GiB
+    # untiled) runs the full- and half-resolution stages in one-frame tiles, except on the FP8 tier (3.9 GiB untiled).
     UNTILED_MAX_BYTES = TILED_MAX_BYTES = 4.5 * GiB
 
-    def __init__(self, encoder: Encoder3d, conv1: nn.Module, mean: torch.Tensor, std: torch.Tensor):
+    def __init__(self, encoder: Encoder3d, conv1: nn.Module, mean: torch.Tensor, std: torch.Tensor,
+                 quant: Optional[str] = None):
         self.encoder, self.conv1_mod, self.mean, self.std = encoder, conv1, mean, std
         self._tile_override: Optional[int] = None     # frames per tile instead of the budget's choice (tests)
+        # None: fp16 / bf16 everywhere; "fp8": residual.2 / residual.6 of every ResidualBlock and head.2 run on e4m3
+        # inputs and weights (fp16 only).  Part of the prepared-weights key: switching rebuilds the buffers.
+        self.quant = quant
         self._key = None
         self.initialised = False
 
     def _prepare(self, dtype, device, H, W):
+        if self.quant not in (None, "fp8"):
+            raise ValueError(f"VAE encoder quant must be 'fp8' or None, got {self.quant!r}")
+        if self.quant == "fp8" and dtype != torch.float16:
+            raise ValueError(f"the FP8 VAE tier runs in float16, got {dtype}")
         e = self.encoder
-        key = (dtype, str(device), H, W, _weights_tag(e.conv1.weight), self._tile_override)
+        key = (dtype, str(device), H, W, _weights_tag(e.conv1.weight), self.quant, self._tile_override)
         if self._key == key:
             return
         pc = lambda m, **kw: _prep_conv(m.weight.data, m.bias.data, dtype, device, **kw)  # noqa: E731
@@ -840,6 +848,12 @@ class EncoderEngine(_StreamLedger):
                 self.blocks.append(d)
         self.g_head = g(e.head[0])
         self.head = pc(e.head[2])
+        if self.quant == "fp8":
+            for b in self.blocks:
+                if b["kind"] == "res":
+                    _to_fp8(b["c1"], b["g1"])
+                    _to_fp8(b["c2"], b["g2"])
+            _to_fp8(self.head, self.g_head)
         self.w_out = self.conv1_mod.weight.data.reshape(32, 32).to(device=device, dtype=dtype).contiguous()
         self.b_out = self.conv1_mod.bias.data.to(device=device, dtype=dtype).contiguous()
         self.mean_d = self.mean.to(device=device, dtype=dtype)
@@ -866,7 +880,8 @@ class EncoderEngine(_StreamLedger):
         plan = []
 
         def buf(conv: _Conv, t, h, w):
-            plan.append((conv, (2 + t, h, w, conv.cin), self.dtype))
+            plan.append((conv, (2 + t, h, w, conv.cin),
+                         torch.float8_e4m3fn if conv.in_scale is not None else self.dtype))
 
         t = min(tile, self.MAX_CHUNK)
         buf(self.conv_in, t, H, W)
@@ -917,12 +932,21 @@ class EncoderEngine(_StreamLedger):
             return
         self.initialised = True
 
-    def _conv(self, c: _Conv, T, src=None, **kw):
+    def _conv(self, c: _Conv, T, src=None, norm_scale: Optional[float] = None, **kw):
         x = c.buf if src is None else src
-        ops.vae_conv(x, c.weight, c.bias, n=c.n, cout=c.cout, T=T, taps=c.taps,
-                     tile=_tile_for(x.shape[1], x.shape[2]), **kw)
+        out_norm = kw.get("out_norm")
+        if x.dtype == torch.float8_e4m3fn or (out_norm is not None and out_norm.dtype == torch.float8_e4m3fn):
+            # FP8 tier: an e4m3 conv, or a 16-bit conv writing the e4m3 input of the next one
+            ops.vae_conv_fp8(x, c.weight, c.bias, n=c.n, cout=c.cout, T=T, taps=c.taps,
+                             tile=_tile_for(x.shape[1], x.shape[2]), w_scale=c.w_scale, in_scale=c.in_scale,
+                             norm_scale=norm_scale, **kw)
+        else:
+            ops.vae_conv(x, c.weight, c.bias, n=c.n, cout=c.cout, T=T, taps=c.taps,
+                         tile=_tile_for(x.shape[1], x.shape[2]), **kw)
         if src is None and c.taps[0] == 3:
-            ops.kv_roll(c.buf.view(c.buf.shape[0], -1), 0, T, 2)     # roll the feature cache (see DecoderEngine._conv)
+            # roll the feature cache (see DecoderEngine._conv); e4m3 buffers move as 16-bit pairs
+            buf = c.buf.view(torch.float16) if c.buf.dtype == torch.float8_e4m3fn else c.buf
+            ops.kv_roll(buf.view(buf.shape[0], -1), 0, T, 2)
 
     # -- one chunk ---------------------------------------------------------------------------------
     def encode_chunk(self, frames: torch.Tensor, first: bool) -> torch.Tensor:
@@ -939,7 +963,8 @@ class EncoderEngine(_StreamLedger):
             h, w = self.H, self.W
             cin.buf[2:2 + t, :, :, :3] = frames[f0:f0 + t].to(self.dtype).permute(0, 2, 3, 1)
             x = self._new(t, h, w, cin.cout)
-            self._conv(cin, t, out_raw=x, out_norm=blocks[0]["c1"].buf[2:2 + t], gamma=blocks[0]["g1"])
+            nxt = blocks[0]["c1"]
+            self._conv(cin, t, out_raw=x, out_norm=nxt.buf[2:2 + t], gamma=blocks[0]["g1"], norm_scale=nxt.in_scale)
             for i in range(s):
                 x, t, h, w = self._block(i, x, t, h, w, first)
             h, w = h // 2, w // 2
@@ -974,17 +999,21 @@ class EncoderEngine(_StreamLedger):
             if b["sc"] is not None:
                 res = self._new(T, h, w, b["cout"])
                 self._conv(b["sc"], T, src=x, out_raw=res)
-            self._conv(b["c1"], T, out_norm=b["c2"].buf[2:2 + T], gamma=b["g2"])
+            self._conv(b["c1"], T, out_norm=b["c2"].buf[2:2 + T], gamma=b["g2"], norm_scale=b["c2"].in_scale)
             g, nxt = self._next_norm(i)
             need_raw = nxt is not self.head
             xo = self._new(T, h, w, b["cout"]) if need_raw else None
             self._conv(b["c2"], T, residual=res, out_raw=xo,
-                       out_norm=nxt.buf[2:2 + T] if g is not None else None, gamma=g)
+                       out_norm=nxt.buf[2:2 + T] if g is not None else None, gamma=g,
+                       norm_scale=nxt.in_scale if g is not None else None)
             return xo, T, h, w
         if b["kind"] == "attn":
             x = _vae_attention(b, x)
             nb = self.blocks[i + 1]
-            ops.vae_rmsnorm_silu(x, nb["g1"], nb["c1"].buf[2:2 + T])
+            if nb["c1"].in_scale is not None:
+                ops.vae_rmsnorm_silu_fp8(x, nb["g1"], nb["c1"].buf[2:2 + T], nb["c1"].in_scale)
+            else:
+                ops.vae_rmsnorm_silu(x, nb["g1"], nb["c1"].buf[2:2 + T])
             return x, T, h, w
         h, w = h // 2, w // 2
         if b["mode"] != "downsample3d":
@@ -1003,7 +1032,7 @@ class EncoderEngine(_StreamLedger):
         if b["mode"] != "downsample3d" or first:
             g, nxt = self._next_norm(i)
             self._conv(b["conv"], T, src=x, out_raw=out[f0:f0 + T], out_norm=nxt.buf[2 + f0:2 + f0 + T], gamma=g,
-                       sub2=True)
+                       norm_scale=nxt.in_scale, sub2=True)
         else:
             self._conv(b["conv"], T, src=x, out_raw=out[f0:f0 + T], sub2=True)
 
@@ -1022,8 +1051,8 @@ class EncoderEngine(_StreamLedger):
         T2 = T // 2
         xo = self._new(T2, h, w, C)
         for j in range(T2):
-            ops.vae_conv(xin[2 * j:2 * j + 3], tc.weight, tc.bias, n=tc.n, cout=tc.cout, T=1, taps=tc.taps,
-                         tile=_tile_for(h, w), out_raw=xo[j:j + 1], out_norm=nxt.buf[2 + j:3 + j], gamma=g)
+            self._conv(tc, 1, src=xin[2 * j:2 * j + 3], out_raw=xo[j:j + 1], out_norm=nxt.buf[2 + j:3 + j], gamma=g,
+                       norm_scale=nxt.in_scale)
         return xo, T2
 
     def encode_first(self, frame: torch.Tensor) -> torch.Tensor:
@@ -1033,6 +1062,10 @@ class EncoderEngine(_StreamLedger):
 
     def encode(self, z: torch.Tensor, feat_cache, stream: bool = False):
         """The wrapper loop of vae_block3.py:141-165: z [3, T, H, W] -> mu [16, T', H/8, W/8]."""
+        if feat_cache is not None and any(
+                c is not None and m is not None and (c.dtype == torch.float8_e4m3fn) != (m.dtype == torch.float8_e4m3fn)
+                for c, m in zip(feat_cache, self._views())):
+            feat_cache = None        # a cache of the other tier (quant was switched): its values do not carry over
         self.import_cache(feat_cache)
         t = z.shape[1]
         outs = []
@@ -1074,6 +1107,9 @@ class VAEEncoderWrapper(nn.Module):
         self.register_buffer("std", torch.tensor(STD, dtype=torch.float32))
         self.z_dim = 16
         self._engine: Optional[EncoderEngine] = None
+        # "fp8": the FP8 (e4m3) tier of the normalised-input convs (fp16 only); KR_VAE_ENC_FP8=1 turns it on by
+        # default.  Switching the tier rebuilds the engine's buffers: the next call starts a new stream.
+        self.quant: Optional[str] = _default_quant("KR_VAE_ENC_FP8")
 
     def _apply(self, fn, *a, **k):
         self._engine = None
@@ -1086,6 +1122,7 @@ class VAEEncoderWrapper(nn.Module):
         if self._engine is None:
             self._engine = EncoderEngine(self.encoder, self.conv1, self.mean, self.std)
         eng = self._engine
+        eng.quant = self.quant
         dtype = z.dtype if z.dtype in (torch.float16, torch.bfloat16) else torch.float16
         eng._prepare(dtype, z.device, z.shape[-2], z.shape[-1])
         mu = eng.encode(z[0], list(feat_cache), stream=stream)
