@@ -525,25 +525,24 @@ int gemm_tn(int dtype, int epi, const void* a, int lda, const void* w, int ldw, 
     set_last_error("gemm: residual epilogue without residual pointer");
     return KR_ERR_INVALID_ARG;
   }
+  // the epilogues read residual and gate rows as 16-byte vectors, like the output rows
+  if ((epi == EPI_BIAS_GATE_RES || epi == EPI_BIAS_RES || epi == EPI_MUL) && p.ldr % 8 != 0) {
+    set_last_error("gemm: unsupported residual pitch ldr=%d (need ldr %% 8 == 0)", p.ldr);
+    return KR_ERR_UNSUPPORTED_SHAPE;
+  }
   if (p.out2 != nullptr && (p.n_split % 256 != 0 || p.ldc2 % 8 != 0 || epi == EPI_F32)) {
     set_last_error("gemm: split output needs n_split %% 256 == 0, ldc2 %% 8 == 0 and a 16-bit epilogue");
     return KR_ERR_INVALID_ARG;
   }
-  if (epi == EPI_BIAS_GATE_RES && (p.gate == nullptr || p.rows_per_gate <= 0)) {
-    set_last_error("gemm: gate epilogue without gate pointer / rows_per_gate");
+  if (epi == EPI_BIAS_GATE_RES && (p.gate == nullptr || p.rows_per_gate <= 0 || p.gate_stride % 8 != 0)) {
+    set_last_error("gemm: gate epilogue without gate pointer / rows_per_gate, or gate stride %% 8 != 0");
     return KR_ERR_INVALID_ARG;
   }
   const bool have_ws = workspace != nullptr && workspace_bytes >= gemm_sk_workspace_bytes();
   const int plan = gemm_plan(epi, p.M, p.N, p.K, have_ws);
   if (plan == 2) return gemm_sk_tn(dtype, epi, a, lda, w, ldw, p, workspace, workspace_bytes, stream);
   if (plan == 1) return gemm2_tn(dtype, epi, a, lda, w, ldw, p, stream);
-  if (plan == 3) {
-    if (p.out2 != nullptr && p.n_split % 32 != 0) {
-      set_last_error("gemm: split output needs n_split %% 32 == 0");
-      return KR_ERR_INVALID_ARG;
-    }
-    return gemm_flex(dtype, epi, a, lda, w, ldw, p, gemm_flex_bn(epi, p.M, p.N, p.K), stream);
-  }
+  if (plan == 3) return gemm_flex(dtype, epi, a, lda, w, ldw, p, gemm_flex_bn(epi, p.M, p.N, p.K), stream);
   return gemm_single(dtype, epi, a, lda, w, ldw, p, stream);
 }
 

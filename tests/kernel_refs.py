@@ -17,7 +17,7 @@ from oracle import dit_oracle as O
 from oracle import vae_oracle as V
 
 F64 = torch.float64
-_MANT = {torch.bfloat16: 7, torch.float16: 10}
+_MANT = {torch.bfloat16: 7, torch.float16: 10, torch.float32: 23}
 
 
 def r16(x: torch.Tensor, dtype=torch.bfloat16) -> torch.Tensor:
@@ -174,3 +174,210 @@ def vae_rmsnorm_silu(x, gamma, dtype):
 
 def softmax_rows(s):
     return torch.softmax(s.double(), dim=-1)
+
+
+# ---------------------------------------------------------------------------------------------
+# kr_gemm.cu, kr_gemm2.cu, kr_gemm_sk.cu, kr_gemm_fp8.cu (gemm_epilogue_row's rounding points)
+# ---------------------------------------------------------------------------------------------
+EPI_BIAS, EPI_BIAS_GELU, EPI_BIAS_GATE_RES, EPI_BIAS_RES, EPI_F32, EPI_MUL = 0, 1, 2, 3, 4, 5
+EPI_NAMES = {EPI_BIAS: "bias", EPI_BIAS_GELU: "gelu", EPI_BIAS_GATE_RES: "gate_res", EPI_BIAS_RES: "res",
+             EPI_F32: "f32", EPI_MUL: "mul"}
+# The accumulation bound E = c_acc * (|a| |w|^T) of one kernel family, float64 operands decoded exactly.  Largest
+# ratio observed on an H100 SXM (700 W) by tests/test_gemm_parity_gpu.py: 3.7e-6 = 2^-18.0 for 16-bit operands (the
+# VAE's P V at K = 14400; <= 8.6e-7 at K <= 5120), 6.4e-5 = 2^-13.9 for e4m3 with per-k-block promotion.  Each
+# constant is >= 4x that; a dropped k-block of unit-variance operands at K = 5120 exceeds E_16 > 100-fold (median) and
+# E_e4m3 on most elements.
+C_ACC_16 = 2.0 ** -16
+C_ACC_E4M3 = 2.0 ** -11
+# the fp32 operations between the accumulator and the first 16-bit rounding (scales, bias add), relative
+F32_EPI = 2.0 ** -22
+# the fp32 tanhf GELU of the kernel: absolute error bound (a few ulps of 1 + tanh, times x / 2) and the largest
+# fraction of elements allowed to round to a neighbour of the float64 GELU
+_GELU_ABS = 2.0 ** -21
+GELU_MAX_FRAC = 5e-3
+GELU_ARGMIN, GELU_MIN = -0.7524614212122512, -0.170040750571254
+# guard buffers: bits no kernel writes (a NaN in bf16, fp16 and fp32)
+SENTINEL16, SENTINEL32 = 0x7E5A, 0x7FC0DEAD
+GUARD_ROWS, GUARD_COLS = 3, 8
+
+
+def gemm_interval(a, w, bias=None, row_scale=None, col_scale=None, c_acc=C_ACC_16):
+    """(z, m, E) in float64 on the device of the operands: z = (a w^T) [* row_scale[m]] [* col_scale[n]] + bias,
+    m = |a| |w|^T with the same scales, and the bound E = c_acc * m + 2^-22 (|z| + |bias|) that the kernel's fp32
+    result before its first 16-bit rounding must lie within.  ``a`` / ``w`` are already decoded to a float type
+    (e4m3 operands decode exactly); ``col_scale`` may be a Python float (the per-tensor FP8 scale)."""
+    a64, w64 = a.double(), w.double()
+    z = a64 @ w64.t()
+    m = a64.abs() @ w64.abs().t()
+    if row_scale is not None:
+        rs = row_scale.double().view(-1, 1)
+        z, m = z * rs, m * rs.abs()
+    if col_scale is not None:
+        cs = col_scale.double().view(1, -1) if torch.is_tensor(col_scale) else float(col_scale)
+        z = z * cs
+        m = m * (cs.abs() if torch.is_tensor(cs) else abs(cs))
+    babs = 0.0
+    if bias is not None:
+        z = z + bias.double()
+        babs = bias.double().abs()
+    return z, m, c_acc * m + F32_EPI * (z.abs() + babs)
+
+
+def _bits_neighbour(y: torch.Tensor, up: torch.Tensor, dtype) -> torch.Tensor:
+    """The 16-bit value adjacent to y (float64 holding dtype values) above it where ``up``, below it elsewhere."""
+    b = y.to(dtype).view(torch.int16).to(torch.int32)
+    o = torch.where(b < 0, -(b & 0x7FFF), b)                      # sign-magnitude -> ordered integers
+    o = o + torch.where(up, 1, -1)
+    b = torch.where(o < 0, (-o) | 0x8000, o).to(torch.int16)    # -0 and +0 are one step apart here: harmless
+    return b.view(dtype).to(F64)
+
+
+def acc_ratio(y16, z, m, dtype) -> float:
+    """Largest c for which y16 = r16(acc + b) needs |acc + b - z| >= c * m: the distance from z to the rounding
+    boundary nearest to it on y16's side, over m, for the elements where y16 != r16(z) (0 elsewhere)."""
+    y = y16.double()
+    off = y != r16(z, dtype)
+    if not bool(off.any()):
+        return 0.0
+    y, zz, mm = y[off], z[off], m[off]
+    mid = 0.5 * (y + _bits_neighbour(y, y < zz, dtype))
+    return float(((mid - zz).abs() / mm.clamp_min(1e-300)).max())
+
+
+def gelu_interval(lo, hi):
+    """[min, max] of GELU-tanh over [lo, hi] (float64): monotone except for its minimum at GELU_ARGMIN."""
+    g_lo, g_hi = gelu_tanh(lo), gelu_tanh(hi)
+    mn = torch.minimum(g_lo, g_hi)
+    mn = torch.where((lo < GELU_ARGMIN) & (hi > GELU_ARGMIN), torch.full_like(mn, GELU_MIN), mn)
+    return mn, torch.maximum(g_lo, g_hi)
+
+
+def gate_rows(M, gate, rows_per_gate, row_offset, device):
+    """gate[(row + row_offset) // rows_per_gate] for rows [0, M), float64."""
+    g = (torch.arange(M, device=device) + row_offset) // rows_per_gate
+    return gate.double()[g]
+
+
+def epi_chain(epi, y16, dtype, residual=None, gate_r=None):
+    """gemm_epilogue_row on the rounded first value y16 = r16(acc + b) (float64), with the kernel's rounding points:
+    r16(gelu(y16)), r16(res + r16(y16 * g)), r16(res + y16), r16(y16 * res).  Exact for every epilogue but GELU
+    (the products and sums of two 16-bit values are exact in fp32); for GELU the unrounded float64 value."""
+    if epi == EPI_BIAS:
+        return y16
+    if epi == EPI_BIAS_GELU:
+        return gelu_tanh(y16)
+    res = residual.double()
+    if epi == EPI_BIAS_GATE_RES:
+        return r16(res + r16(y16 * gate_r, dtype), dtype)
+    if epi == EPI_BIAS_RES:
+        return r16(res + y16, dtype)
+    if epi == EPI_MUL:
+        return r16(y16 * res, dtype)
+    raise ValueError(epi)
+
+
+def _mul_interval(lo, hi, f):
+    a, b = lo * f, hi * f
+    return torch.minimum(a, b), torch.maximum(a, b)
+
+
+def chain_interval(epi, lo, hi, dtype, residual=None, gate_r=None):
+    """The epilogue chain applied to both ends of y16's interval [lo, hi] (every step monotone on it, or bounded by
+    its extremum), so that any correct kernel's output lies inside the returned [lo, hi]."""
+    if epi == EPI_BIAS:
+        return lo, hi
+    if epi == EPI_BIAS_GELU:
+        g_lo, g_hi = gelu_interval(lo, hi)
+        return (r16(g_lo - _GELU_ABS * lo.abs().maximum(hi.abs()), dtype),
+                r16(g_hi + _GELU_ABS * lo.abs().maximum(hi.abs()), dtype))
+    res = residual.double()
+    if epi == EPI_BIAS_GATE_RES:
+        p_lo, p_hi = _mul_interval(lo, hi, gate_r)
+        return r16(res + r16(p_lo, dtype), dtype), r16(res + r16(p_hi, dtype), dtype)
+    if epi == EPI_BIAS_RES:
+        return r16(res + lo, dtype), r16(res + hi, dtype)
+    if epi == EPI_MUL:
+        p_lo, p_hi = _mul_interval(lo, hi, res)
+        return r16(p_lo, dtype), r16(p_hi, dtype)
+    raise ValueError(epi)
+
+
+def _outside(got, lo, hi, scale):
+    """Largest distance of got outside [lo, hi], in units of ``scale`` (0 when every element is inside)."""
+    d = (lo - got).clamp_min(0) + (got - hi).clamp_min(0)
+    return float((d / scale).max()) if d.numel() else 0.0
+
+
+def check_gemm(epi, got, z, m, E, dtype, *, residual=None, gate_r=None, alpha=1.0, y16=None):
+    """Hold one GEMM output to the float64 reference.  Returns (violations, stats).
+
+    got: the kernel's output (16-bit, or fp32 for EPI_F32).  z, m, E: :func:`gemm_interval`.  y16: the EPI_BIAS
+    output of the SAME kernel on the same operands (same accumulation order), when the planner sent both there; the
+    rest of the chain is then checked exactly (GELU: within the fp32 tanhf error on all elements, and not
+    bit-identical on at most GELU_MAX_FRAC of them).  Every epilogue is also checked against the accumulation
+    interval carried through the chain.  stats: ``excess`` (ulps outside the interval), ``frac`` (elements not equal
+    to the chain applied to r16(z)), ``ratio`` (:func:`acc_ratio`, first-rounding epilogues only)."""
+    viol = []
+    g = got.double()
+    if not bool(torch.isfinite(g).all()):
+        viol.append("non-finite output")
+        g = torch.nan_to_num(g, nan=1e300)
+    if epi == EPI_F32:
+        lo, hi = (z - E) * alpha, (z + E) * alpha
+        u = ulp(torch.maximum(lo.abs(), hi.abs()), torch.float32)
+        ex = _outside(g, lo - 2 * u, hi + 2 * u, u)
+        if ex > 0:
+            viol.append(f"f32: {ex:.3g} fp32 ulps outside [(z-E)a, (z+E)a] widened by 2 ulps")
+        d = (g / alpha - z).abs() if alpha != 0 else (g - z).abs()
+        ratio = float(((d - 2 * u / abs(alpha)).clamp_min(0) / m.clamp_min(1e-300)).max())
+        return viol, {"excess": ex, "frac": float((g != (z * alpha).float().double()).double().mean()),
+                      "ratio": ratio}
+    lo, hi = r16(z - E, dtype), r16(z + E, dtype)
+    c_lo, c_hi = chain_interval(epi, lo, hi, dtype, residual, gate_r)
+    ex = _outside(g, c_lo, c_hi, ulp(g, dtype))
+    if ex > 0:
+        viol.append(f"{EPI_NAMES[epi]}: {ex:.3g} ulps outside the accumulation interval")
+    nearest = epi_chain(epi, r16(z, dtype), dtype, residual, gate_r)
+    stats = {"excess": ex, "frac": float((g != r16(nearest, dtype)).double().mean())}
+    if epi == EPI_BIAS:
+        stats["ratio"] = acc_ratio(g, z, m, dtype)
+    if y16 is not None:
+        want = epi_chain(epi, y16.double(), dtype, residual, gate_r)
+        if epi == EPI_BIAS_GELU:
+            s = _GELU_ABS * y16.double().abs()
+            ex2 = _outside(g, r16(want - s, dtype), r16(want + s, dtype), ulp(g, dtype))
+            fr = float((g != r16(want, dtype)).double().mean())
+            stats["chain_frac"] = fr
+            if ex2 > 0 or fr > GELU_MAX_FRAC:
+                viol.append(f"gelu chain: {ex2:.3g} ulps outside the fp32 GELU error, {fr:.3g} not bit-identical")
+        else:
+            bad = int((g != want).sum())
+            stats["chain_frac"] = bad / max(1, g.numel())
+            if bad:
+                viol.append(f"{EPI_NAMES[epi]} chain: {bad} elements differ from the exact restatement")
+    return viol, stats
+
+
+def guarded(rows: int, cols: int, dtype, device, fill=None):
+    """A [rows, cols] view inside a sentinel-filled buffer with GUARD_ROWS rows above and below and GUARD_COLS + 16
+    columns beside it (row pitch cols + 24 > cols, 16-byte aligned).  ``fill``, if given, is copied into the view."""
+    buf = torch.empty(rows + 2 * GUARD_ROWS, cols + 3 * GUARD_COLS, dtype=dtype, device=device)
+    if dtype == torch.float32:
+        buf.view(torch.int32).fill_(SENTINEL32)
+    else:
+        buf.view(torch.int16).fill_(SENTINEL16)
+    view = buf[GUARD_ROWS:GUARD_ROWS + rows, GUARD_COLS:GUARD_COLS + cols]
+    if fill is not None:
+        view.copy_(fill)
+    return buf, view
+
+
+def guard_intact(buf: torch.Tensor, rows: int, cols: int) -> bool:
+    """True when every element of ``buf`` outside the view of :func:`guarded` still holds the sentinel."""
+    if buf.dtype == torch.float32:
+        bits, s = buf.view(torch.int32), SENTINEL32
+    else:
+        bits, s = buf.view(torch.int16), SENTINEL16
+    keep = torch.ones(bits.shape, dtype=torch.bool, device=buf.device)
+    keep[GUARD_ROWS:GUARD_ROWS + rows, GUARD_COLS:GUARD_COLS + cols] = False
+    return bool((bits[keep] == s).all())
