@@ -220,8 +220,11 @@ int kr_unpatchify_x0(const void* head_out, int ldh, const void* xt, const double
  *   out_raw  = cast(acc + bias [+ residual])
  *   out_norm = SiLU(RMS_norm_C(out_raw) * sqrt(cout) * gamma)     (vae.py:39-54, :184-186)
  *   out_pix  = clamp(out_raw, -1, 1) as fp32 [T, cout, H, W]       (vae_block3.py:226)
+ * out_pix is the output of n = 16 (the head) and its only one: out_pix with n != 16, or out_raw,
+ * out_norm or residual with n = 16, is KR_ERR_INVALID_ARG.
  * sub2 = 1: the encoder's stride-2 Conv2d behind ZeroPad2d((0,1,0,1)) (vae.py:84-92): only the odd
- * (h, w) positions of the stride-1 result are kept, compacted to an H/2 x W/2 output.
+ * (h, w) positions of the stride-1 result are kept, compacted to an H/2 x W/2 output.  It needs
+ * (kt, kh, kw) = (1, 3, 3) and no out_pix (KR_ERR_INVALID_ARG otherwise).
  * Extra (cin, n) pairs for the encoder: (64,96) (96,192) (384,32). */
 int kr_vae_conv3d(int dtype, int cin, int n, const void* in, int t_in, const void* weight,
                   int w_rows, const void* bias, int cout, int T, int H, int W, int tile_w, int tile_h,

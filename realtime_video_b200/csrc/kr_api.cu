@@ -281,6 +281,12 @@ int kr_vae_conv3d(int dtype, int cin, int n, const void* in, int t_in, const voi
   KR_REQUIRE(in && weight, "null input/weight");
   KR_REQUIRE(dtype == 0 || dtype == 1, "dtype must be 0 (bf16) or 1 (fp16)");
   KR_REQUIRE(out_raw || out_norm || out_pix, "no output requested");
+  // the epilogue writes pixels only for the 16-channel head, and the head writes nothing else
+  KR_REQUIRE(!out_pix || n == 16, "out_pix is the n = 16 head's output");
+  KR_REQUIRE(n != 16 || (!out_raw && !out_norm && !residual), "the n = 16 head takes no out_raw/out_norm/residual");
+  // sub2 keeps the odd positions of the stride-1 3x3 conv: that is the stride-2 conv behind ZeroPad2d((0,1,0,1))
+  // only for (1, 3, 3) taps, and the pixel store does not halve the plane
+  KR_REQUIRE(!sub2 || (kt == 1 && kh == 3 && kw == 3 && !out_pix), "sub2 is the (1,3,3) stride-2 conv without out_pix");
   kr::ConvParams p;
   p.T = T; p.H = H; p.W = W; p.TW = tile_w; p.TH = tile_h; p.KT = kt; p.KH = kh; p.KW = kw;
   p.cout = cout;

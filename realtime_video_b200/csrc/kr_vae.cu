@@ -1343,6 +1343,9 @@ static int vae_conv_fp8_entry(int in_fp8, int cin, int n, const void* in, int t_
   KR_VAE_F8_REQUIRE(t_in >= T + kt - 1, "input holds too few frames");
   KR_VAE_F8_REQUIRE(!sub2 || (!in_fp8 && out_pix == nullptr && kt == 1 && kh == 3 && kw == 3),
                     "sub2 is the 16-bit 3x3 stride-2 conv");
+  KR_VAE_F8_REQUIRE(!out_pix || n == 16, "out_pix is the n = 16 head's output");
+  KR_VAE_F8_REQUIRE(n != 16 || (!out_raw && !out_norm && !residual),
+                    "the n = 16 head takes no out_raw/out_norm/residual");
   kr::ConvParams p;
   p.T = T; p.H = H; p.W = W; p.TW = tile_w; p.TH = tile_h; p.KT = kt; p.KH = kh; p.KW = kw;
   p.cout = cout;

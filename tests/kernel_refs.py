@@ -381,3 +381,129 @@ def guard_intact(buf: torch.Tensor, rows: int, cols: int) -> bool:
     keep = torch.ones(bits.shape, dtype=torch.bool, device=buf.device)
     keep[GUARD_ROWS:GUARD_ROWS + rows, GUARD_COLS:GUARD_COLS + cols] = False
     return bool((bits[keep] == s).all())
+
+
+# ---------------------------------------------------------------------------------------------
+# kr_vae.cu conv_igemm_kernel / conv_halo_kernel (conv_epilogue_frag's rounding points)
+# ---------------------------------------------------------------------------------------------
+# the fused RMS_norm -> SiLU of the epilogue against vae_rmsnorm_silu on the kernel's own raw values: not bit-identical
+# (fp32 sum of squares, a multiply by the fp32 reciprocal of the norm instead of a division, __expf) on at most
+# NORM_MAX_FRAC of the elements.  A 1-ulp difference at one of the three 16-bit roundings before the SiLU grows to a few
+# ulps of the output where SiLU is small against its argument (x < 0), so at most NORM_FAR_FRAC of the elements may be
+# more than 1 ulp away, and none more than NORM_FAR_ULPS.  An emulation of the kernel's fp32 arithmetic on 3.8e7
+# random elements shows 6 ulps on 9e-6 of them; on an H100 SXM (700 W) the worst was 5 ulps, with 4.3e-4 of the
+# elements not bit-identical.
+NORM_MAX_FRAC, NORM_FAR_FRAC, NORM_FAR_ULPS = 2e-2, 1e-4, 8
+CONV_FORMS = ("raw", "res", "norm", "head")
+
+
+def conv_interval(x, w5, bias, taps, sub2=False, T=None, c_acc=C_ACC_16, frames_per_chunk=4):
+    """(z, m, E) float64 [T, Ho, Wo, rows] of the causal conv on the device of its operands.
+
+    x [t_in, H, W, cin] holds the kt - 1 history frames in front of the T new ones (T defaults to t_in - kt + 1; frames
+    past T + kt - 1 are not read); w5 [rows, kt, kh, kw, cin] (the kernel's weight [rows, taps*cin] viewed); H / W are
+    zero padded by kh // 2, kw // 2.  ``sub2``: ZeroPad2d((0,1,0,1)) then the stride-2 conv (vae.py:84-92), output
+    H // 2 x W // 2.  m is the same conv of |x| and |w|, and E = c_acc m + 2^-22 (|z| + |b|)."""
+    kt, kh, kw = taps
+    rows = w5.shape[0]
+    T = x.shape[0] - kt + 1 if T is None else T
+    wd = w5.double().reshape(rows, kt, kh, kw, -1).permute(0, 4, 1, 2, 3)
+    zs, ms = [], []
+    for t0 in range(0, T, frames_per_chunk):
+        t1 = min(T, t0 + frames_per_chunk)
+        xd = x[t0:t1 + kt - 1].double().permute(3, 0, 1, 2)[None]
+        if sub2:
+            assert (kh, kw) == (3, 3)
+            pad, stride = (0, 1, 0, 1, 0, 0), (1, 2, 2)
+        else:
+            pad, stride = (kw // 2, kw // 2, kh // 2, kh // 2, 0, 0), 1
+        zs.append(F.conv3d(F.pad(xd, pad), wd, stride=stride)[0].permute(1, 2, 3, 0))
+        ms.append(F.conv3d(F.pad(xd.abs(), pad), wd.abs(), stride=stride)[0].permute(1, 2, 3, 0))
+        del xd
+    z, m = torch.cat(zs), torch.cat(ms)
+    babs = 0.0
+    if bias is not None:
+        z = z + bias[:rows].double()
+        babs = bias[:rows].double().abs()
+    return z, m, c_acc * m + F32_EPI * (z.abs() + babs)
+
+
+def check_conv(form, got, z, m, E, dtype, *, y16=None, residual=None, gamma=None, cout=None):
+    """Hold one conv output to the float64 reference.  Returns (violations, stats) as :func:`check_gemm`.
+
+    raw:  r16(acc + b) inside [r16(z - E), r16(z + E)] (stats["ratio"]: :func:`acc_ratio`).
+    res:  r16(res + r16(acc + b)): inside the interval carried through the add, and equal to r16(res + y16) exactly,
+          y16 the raw-only output of the same kernel on the same operands.
+    norm: SiLU(RMS_norm(raw) * sqrt(cout) * gamma) on the kernel's own raw values ``y16`` (the raw, or raw + residual,
+          output of the same launch form): channels < cout within 1 ulp of :func:`vae_rmsnorm_silu` but for
+          NORM_FAR_FRAC of them (<= NORM_FAR_ULPS), not bit-identical on at most NORM_MAX_FRAC; channels >= cout (zero
+          weight rows) exactly 0.
+    head: clamp(r16(acc + b), -1, 1) as fp32, ``got`` [T, Ho, Wo, cout] (the NCHW output permuted), z of the first
+          cout channels."""
+    viol = []
+    if form == "raw":
+        return check_gemm(EPI_BIAS, got, z, m, E, dtype)
+    if form == "res":
+        return check_gemm(EPI_BIAS_RES, got, z, m, E, dtype, residual=residual, y16=y16)
+    g = got.double()
+    if not bool(torch.isfinite(g).all()):
+        viol.append("non-finite output")
+        g = torch.nan_to_num(g, nan=1e300)
+    if form == "head":
+        c = g.shape[-1]
+        lo = r16(z[..., :c] - E[..., :c], dtype).clamp(-1, 1)
+        hi = r16(z[..., :c] + E[..., :c], dtype).clamp(-1, 1)
+        ex = _outside(g, lo, hi, ulp(g, dtype))
+        if ex > 0:
+            viol.append(f"head: {ex:.3g} ulps outside the clamped accumulation interval")
+        nearest = r16(z[..., :c], dtype).clamp(-1, 1)
+        inner = (g > -1) & (g < 1)
+        ratio = acc_ratio(torch.where(inner, g, r16(z[..., :c], dtype)), z[..., :c], m[..., :c], dtype)
+        return viol, {"excess": ex, "frac": float((g != nearest).double().mean()), "ratio": ratio}
+    if form == "norm":
+        cout = g.shape[-1] if cout is None else cout
+        want, _ = vae_rmsnorm_silu(y16[..., :cout], gamma[:cout], dtype)
+        du = (g[..., :cout] - want).abs() / ulp(want, dtype)
+        worst = float(du.max())
+        frac, far = float((du != 0).double().mean()), float((du > 1).double().mean())
+        if worst > NORM_FAR_ULPS or far > NORM_FAR_FRAC or frac > NORM_MAX_FRAC:
+            viol.append(f"norm: {worst:.3g} ulps from the restatement on the kernel's raw values, "
+                        f"{far:.3g} more than 1 ulp away, {frac:.3g} not bit-identical")
+        if g.shape[-1] > cout and bool((g[..., cout:] != 0).any()):
+            viol.append("norm: a channel >= cout is not 0")
+        return viol, {"excess": max(0.0, worst - NORM_FAR_ULPS), "frac": frac, "far": far, "worst_ulps": worst}
+    raise ValueError(form)
+
+
+def guarded_frames(T, H, W, C, dtype, device, fill=None, before=1, after=1):
+    """A [T, H, W, C] channels-last view (pixel pitch C + GUARD_COLS, dense rows) inside a sentinel-filled
+    [before + T + after, H, W, C + GUARD_COLS] buffer.  fp32 buffers are [before + T + after, C, H, W] NCHW pixel
+    stacks (``out_pix``): no pitch, a guard frame before and after."""
+    if dtype == torch.float32:
+        buf = torch.empty(before + T + after, C, H, W, dtype=dtype, device=device)
+        buf.view(torch.int32).fill_(SENTINEL32)
+        view = buf[before:before + T]
+    else:
+        buf = torch.empty(before + T + after, H, W, C + GUARD_COLS, dtype=dtype, device=device)
+        buf.view(torch.int16).fill_(SENTINEL16)
+        view = buf[before:before + T, :, :, :C]
+    if fill is not None:
+        view.copy_(fill)
+    return buf, view
+
+
+def frames_intact(buf, T, C, before=1, untouched=()) -> bool:
+    """True when every element of a :func:`guarded_frames` buffer outside its view still holds the sentinel, and so does
+    every frame of the view listed in ``untouched`` (the other half of an interleaved output)."""
+    if buf.dtype == torch.float32:
+        bits, s = buf.view(torch.int32), SENTINEL32
+    else:
+        bits, s = buf.view(torch.int16), SENTINEL16
+    keep = torch.ones(bits.shape, dtype=torch.bool, device=buf.device)
+    if buf.dtype == torch.float32:
+        keep[before:before + T] = False
+    else:
+        keep[before:before + T, :, :, :C] = False
+    for f in untouched:
+        keep[before + f] = True
+    return bool((bits[keep] == s).all())
