@@ -124,7 +124,6 @@ t5_attn_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant
     }
     if (leader) mbar_arrive(&kv_empty[st(2 * j)]);
     // the reference's bf16(bf16(s) + bias), masked keys = finfo.min, key rows past L (TMA zero fill) = -inf
-    float nm[2];
 #pragma unroll
     for (int r = 0; r < 2; ++r) {
       float mt = -INFINITY;
@@ -152,8 +151,10 @@ t5_attn_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant
       }
       l_run[r] *= alpha;
       m_run[r] = m_new;
-      nm[r] = -m_new * kLog2e;
     }
+    // P = exp2((v - m) log2e): v and m are bf16 values, so v - m is exact in fp32, 0 when both are finfo.min (a
+    // tile whose keys are all masked: P = 1, as torch.softmax over equal finfo.min scores; a later real key's
+    // alpha = 0 drops them).  The fused -m * log2e of the usual form overflows to +inf there and makes P = inf.
     uint32_t pa[T5_TK / 16][4];
 #pragma unroll
     for (int kk = 0; kk < T5_TK / 16; ++kk)
@@ -162,8 +163,8 @@ t5_attn_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant
 #pragma unroll
         for (int r = 0; r < 2; ++r) {
           const int i = 8 * kk + 4 * h + 2 * r;
-          const float a0 = fast_exp2(fmaf(s[i], kLog2e, nm[r]));
-          const float a1 = fast_exp2(fmaf(s[i + 1], kLog2e, nm[r]));
+          const float a0 = fast_exp2((s[i] - m_run[r]) * kLog2e);
+          const float a1 = fast_exp2((s[i + 1] - m_run[r]) * kLog2e);
           l_run[r] += a0 + a1;
           pa[kk][2 * h + r] = pack_bf16x2(a0, a1);
         }

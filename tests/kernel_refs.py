@@ -151,6 +151,289 @@ def rel_rows_heads(got, ref, heads):
 
 
 # ---------------------------------------------------------------------------------------------
+# kr_attn.cu attn_fwd_kernel and kr_t5attn.cu t5_attn_kernel: their online-softmax schedules as float64 intervals
+# ---------------------------------------------------------------------------------------------
+# |s - q.k| <= C_S |q|.|k| for the fp32 wgmma scores, |O - sum P v| <= C_PV sum P |v| for the fp32 P V accumulator
+# (carried across tiles and rescales), and the relative error of ex2.approx.ftz.f32 (assumed, not measured: no case
+# needs any).  The smallest values both kernels still pass on an H100 SXM (700 W) are 2^-23 for both C_S and C_PV
+# (tests/test_attn_parity_gpu.py); each constant is 8x that.
+C_S = 2.0 ** -20
+C_PV = 2.0 ** -20
+EXP2_REL = 2.0 ** -21
+U32 = 2.0 ** -24                     # fp32 unit roundoff
+TINY32 = 2.0 ** -126                 # smallest normal fp32: ex2.approx.ftz flushes results below it to 0
+LOG2E_F32 = float(torch.tensor(1.4426950408889634, dtype=torch.float32))   # log2 e as the kernels hold it
+T5_MIN = float(torch.finfo(torch.bfloat16).min)
+ATTN_TILE = 128
+
+
+def f32(x: float) -> float:
+    return float(torch.tensor(x, dtype=torch.float32))
+
+
+def attn_scale_log2(softmax_scale=None) -> float:
+    """kr_attn_fwd's scale_log2 = fp32(scale) * fp32(log2 e), rounded to fp32 (kr_api.cu)."""
+    scale = 1.0 / math.sqrt(128) if softmax_scale is None else softmax_scale
+    return f32(f32(scale) * LOG2E_F32)
+
+
+def attn_rows(Lq, Lkv, block_len=0, window=0, pad_keys=0, device="cpu"):
+    """(row_lo, row_hi, n_phantom) int64 [Lq]: the keys [row_lo, row_hi) each query row sees and the number of padded
+    (phantom) keys it adds in the epilogue, exactly as attn_fwd_kernel derives them."""
+    rows = torch.arange(Lq, device=device)
+    if not block_len:
+        z = torch.zeros_like(rows)
+        return z, z + Lkv, z
+    hi = (rows // block_len + 1) * block_len
+    lo = (hi - window).clamp_min(0) if window > 0 else torch.zeros_like(rows)
+    n_ph = (hi - Lkv).clamp_min(0).clamp_max(pad_keys)
+    return lo, hi.clamp_max(Lkv), n_ph
+
+
+def _exp2_bounds(a_lo, a_hi, c_exp):
+    """[lo, hi] of ex2.approx.ftz(x) for x in [a_lo, a_hi] (float64; results below 2^-126 may be flushed to 0)."""
+    lo = torch.exp2(a_lo) * (1 - c_exp)
+    return torch.where(lo < TINY32, torch.zeros_like(lo), lo), torch.exp2(a_hi) * (1 + c_exp)
+
+
+def _scale_interval(x_lo, x_hi, a_lo, a_hi):
+    """[x_lo, x_hi] * [a_lo, a_hi] for a_lo >= 0, widened by one fp32 rounding of the product."""
+    lo = torch.minimum(x_lo * a_lo, x_lo * a_hi)
+    hi = torch.maximum(x_hi * a_lo, x_hi * a_hi)
+    return lo - U32 * lo.abs(), hi + U32 * hi.abs()
+
+
+def _pv_interval(P_lo, P_hi, v):
+    """[lo, hi] of P v over P in [P_lo, P_hi] (P >= 0) elementwise, and P_hi |v|."""
+    vp, vn = v.clamp_min(0), v.clamp_max(0)
+    return P_lo @ vp + P_hi @ vn, P_hi @ vp + P_lo @ vn, P_hi @ v.abs()
+
+
+def _l_chain(n_tiles, n_rescale):
+    """Relative bound of the fp32 row sum l: each thread adds the pairs a0 + a1 of its 2 columns of every 8 (32 adds
+    per tile), is multiplied by alpha on every rescale, then 2 shuffle adds; every term is >= 0."""
+    return (32 * n_tiles + n_rescale + 4) * U32 * 1.01
+
+
+def _flash_walk(qh, kh, vh, sl2, row_lo, row_hi, dtype, c_s, c_pv, c_exp, rescale_if_ambiguous):
+    """One head of attn_fwd_kernel's tile walk.  Returns the interval state (O_lo, O_hi, A, l_lo, l_hi, mu_lo, mu_hi,
+    n_ambiguous [Lq]): O and l are bounded in the frame of the kernel's own (unknown) m_used, mu = m_used * sl2 in
+    log2 units (-inf while the row has seen no key), A = the P_hi |v| sum behind the C_PV bound."""
+    Lq, dev = qh.shape[0], qh.device
+    inf = torch.tensor(float("inf"), dtype=F64, device=dev)
+    mu_lo = torch.full((Lq,), -float("inf"), dtype=F64, device=dev)
+    mu_hi = mu_lo.clone()
+    O_lo = torch.zeros(Lq, vh.shape[1], dtype=F64, device=dev)
+    O_hi, A = O_lo.clone(), O_lo.clone()
+    l_lo = torch.zeros(Lq, dtype=F64, device=dev)
+    l_hi = l_lo.clone()
+    amb = torch.zeros(Lq, dtype=torch.int64, device=dev)
+    n_resc = torch.zeros(Lq, dtype=torch.int64, device=dev)
+    qa = qh.abs()
+    for k0 in range(0, int(row_hi.max()), ATTN_TILE):
+        k1 = min(k0 + ATTN_TILE, kh.shape[0])
+        cols = torch.arange(k0, k1, device=dev)
+        vis = (cols[None] >= row_lo[:, None]) & (cols[None] < row_hi[:, None])
+        has = vis.any(1)
+        if not bool(has.any()):
+            continue
+        t = (qh @ kh[k0:k1].t()) * sl2
+        dl = (qa @ kh[k0:k1].abs().t()) * (c_s * sl2)
+        t_lo = torch.where(vis, t - dl, -inf)
+        t_hi = torch.where(vis, t + dl, -inf)
+        tmax_lo, tmax_hi = t_lo.amax(1), t_hi.amax(1)
+        # need = fl(fl(m_new - m_run) * sl2) > 8, m_new = max(m_run, tile max); certain on a row's first keys
+        first = has & torch.isinf(mu_lo)
+        D_lo, D_hi = tmax_lo - mu_hi, tmax_hi - mu_lo
+        sure = first | (has & (D_lo * (1 - 4 * U32) > 8))
+        maybe = has & ~sure & (D_hi * (1 + 4 * U32) > 8)
+        amb += maybe.long()
+        resc = sure | (maybe & rescale_if_ambiguous)
+        old = resc & ~first
+        if bool(old.any()):
+            # alpha = ex2(fl(fl(m_run - m_new) * sl2)) on O and l, in the old frame
+            a_lo, a_hi = mu_lo - tmax_hi, mu_hi - tmax_lo
+            al_lo, al_hi = _exp2_bounds(a_lo - 2 * U32 * a_lo.abs(), a_hi + 2 * U32 * a_hi.abs(), c_exp)
+            ol, oh = _scale_interval(O_lo, O_hi, al_lo[:, None], al_hi[:, None])
+            o2 = old[:, None]
+            O_lo, O_hi = torch.where(o2, ol, O_lo), torch.where(o2, oh, O_hi)
+            A = torch.where(o2, A * al_hi[:, None] * (1 + U32), A)
+            l_lo = torch.where(old, l_lo * al_lo, l_lo)
+            l_hi = torch.where(old, l_hi * al_hi, l_hi)
+            n_resc += old.long()
+        mu_lo = torch.where(resc, tmax_lo, mu_lo)
+        mu_hi = torch.where(resc, tmax_hi, mu_hi)
+        # p = ex2.approx(fl(s * sl2 + fl(-m_used * sl2))): both roundings, the key's and the max's own +-delta
+        mabs = torch.maximum(mu_lo.abs(), mu_hi.abs()).nan_to_num(0.0, posinf=0.0)
+        d_lo = t_lo - (mu_hi + U32 * mabs)[:, None]
+        d_hi = t_hi - (mu_lo - U32 * mabs)[:, None]
+        d_lo = torch.where(vis, d_lo - U32 * d_lo.abs(), -inf)
+        d_hi = torch.where(vis, d_hi + U32 * d_hi.abs(), -inf)
+        p_lo, p_hi = _exp2_bounds(d_lo, d_hi, c_exp)
+        P_lo, P_hi = r16(p_lo, dtype), r16(p_hi, dtype)
+        l_lo, l_hi = l_lo + p_lo.sum(1), l_hi + p_hi.sum(1)
+        a, b, c = _pv_interval(P_lo, P_hi, vh[k0:k1])
+        O_lo, O_hi, A = O_lo + a, O_hi + b, A + c
+    n_tiles = (row_hi + ATTN_TILE - 1) // ATTN_TILE
+    g = _l_chain(n_tiles, n_resc).double()
+    return O_lo, O_hi, A, l_lo * (1 - g), l_hi * (1 + g), mu_lo, mu_hi, amb
+
+
+def _flash_epilogue(O_lo, O_hi, A, l_lo, l_hi, mu_lo, mu_hi, n_ph, c_pv, c_exp):
+    """Unrounded [lo, hi] of fl(O * inv_l) with the phantom keys: m_fin = max(m, 0), o_scale = ex2((m - m_fin) sl2),
+    l' = l o_scale + n_ph ex2(-m_fin sl2), inv_l = o_scale / l'  ==  1 / (l + n_ph 2^-mu) for either sign of mu."""
+    E = c_pv * A + 2.0 ** -120
+    O_lo, O_hi = O_lo - E, O_hi + E
+    seen = ~torch.isinf(mu_lo)
+    mabs = torch.where(seen, torch.maximum(mu_lo.abs(), mu_hi.abs()), torch.zeros_like(mu_lo))
+    nph = n_ph.double()
+    ph_lo = torch.where(seen, nph * torch.exp2(-(mu_hi + U32 * mabs)) * (1 - c_exp), nph)
+    ph_hi = torch.where(seen, nph * torch.exp2(-(mu_lo - U32 * mabs)) * (1 + c_exp), nph)
+    den_lo, den_hi = l_lo + ph_lo, l_hi + ph_hi
+    if bool((den_lo <= 0).any()):
+        raise ValueError("attn_interval: a row sees neither a key nor a padded key (its softmax is undefined)")
+    rel = 2 * c_exp + 6 * U32
+    inv_lo, inv_hi = (1 - rel) / den_hi, (1 + rel) / den_lo
+    # ex2 of (m - m_fin) sl2 below -126 flushes o_scale, and with it the row, to 0
+    inv_lo = torch.where((n_ph > 0) & (mu_lo < -125), torch.zeros_like(inv_lo), inv_lo)
+    inv_lo = torch.where(seen, inv_lo, torch.zeros_like(inv_lo))     # no real key: o_scale = 0
+    inv_hi = torch.where(seen, inv_hi, torch.zeros_like(inv_hi))
+    return _scale_interval(O_lo, O_hi, inv_lo[:, None], inv_hi[:, None])
+
+
+def attn_interval(q, k, v, heads, block_len=0, window=0, pad_keys=0, softmax_scale=None, dtype=torch.bfloat16,
+                  head_list=None, *, c_s=C_S, c_pv=C_PV, c_exp=EXP2_REL):
+    """Per-element [lo, hi] (float64 holding ``dtype`` values) of attn_fwd_kernel's 16-bit output, restating its
+    schedule rather than softmax: 128-key tiles in order; scores t = sl2 (q.k) in log2 units with the bound
+    delta = C_S sl2 |q|.|k|; the visible keys [row_lo, row_hi) of :func:`attn_rows`; the lazy running max (rescale only
+    when the tile's max exceeds m_used by more than 8, else P is taken against the stale m_used and may reach 2^8;
+    m_used = -inf until the row's first visible key); p = 2^(t - m_used) with both +-delta, EXP2_REL, the fp32
+    rounding of the fma argument and ftz; P = [r16(p_lo), r16(p_hi)]; l sums the unrounded p (fp32 chain bound of
+    :func:`_l_chain`), O sums P v (C_PV sum P |v|); alpha on a rescale carries its own EXP2_REL; the epilogue of
+    :func:`_flash_epilogue`.  A lazy decision within the error margin of the threshold is ambiguous: the walk runs
+    again deciding every ambiguous tile the other way, and the union is returned (rows with two or more ambiguous tiles
+    are not enumerated over mixed decisions; the count lets a test report them).
+
+    Returns (lo, hi, info) with lo / hi [Lq, len(head_list) * 128] and info: ``u_lo`` / ``u_hi`` (the unrounded
+    bounds), ``ambiguous`` (number of ambiguous tiles), ``heads`` (the restated heads, all by default)."""
+    Lq, Lkv = q.shape[0], k.shape[0]
+    head_list = list(range(heads)) if head_list is None else list(head_list)
+    sl2 = attn_scale_log2(softmax_scale)
+    row_lo, row_hi, n_ph = attn_rows(Lq, Lkv, block_len, window, pad_keys, q.device)
+    us_lo, us_hi, n_amb = [], [], 0
+    for h in head_list:
+        cs = slice(h * 128, (h + 1) * 128)
+        qh, kh, vh = q[:, cs].double(), k[:, cs].double(), v[:, cs].double()
+        lo = hi = None
+        for policy in (False, True):
+            st = _flash_walk(qh, kh, vh, sl2, row_lo, row_hi, dtype, c_s, c_pv, c_exp, policy)
+            a, b = _flash_epilogue(*st[:7], n_ph, c_pv, c_exp)
+            lo = a if lo is None else torch.minimum(lo, a)
+            hi = b if hi is None else torch.maximum(hi, b)
+            n = int(st[7].sum())
+            if not policy:
+                n_amb += n
+            if n == 0:
+                break
+        us_lo.append(lo)
+        us_hi.append(hi)
+    u_lo, u_hi = torch.cat(us_lo, 1), torch.cat(us_hi, 1)
+    return r16(u_lo, dtype), r16(u_hi, dtype), {"u_lo": u_lo, "u_hi": u_hi, "ambiguous": n_amb, "heads": head_list}
+
+
+def t5_attn_interval(q, k, v, bias_delta, key_mask, heads, *, c_s=C_S, c_pv=C_PV, c_exp=EXP2_REL):
+    """Per-element [lo, hi] of t5_attn_kernel's bf16 output [L, heads*64] (head_dim 64, no scaling): per key
+    r16(s) as an interval ([r16(s - C_S |q|.|k|), r16(s + ...)], nearly always one value), then
+    r16(r16(s) + bias[h, k - q + L - 1]); masked keys are finfo.min, keys past L are excluded.  The running max is
+    exact (not lazy) over these bf16 values; p = ex2(fl(fl(v - m) log2e)) (the difference of two bf16 values is exact in
+    fp32) with EXP2_REL and ftz, P = r16(p) un-normalised, l and O in fp32 with the rescale by
+    alpha = ex2(fl(fl(m_run - m_new) log2e)), and out = r16(O / l).  A row whose first tile is masked whole runs that
+    tile's softmax over equal finfo.min values (p = 1) until a real key's alpha = 0 drops it; an all-masked row ends as
+    the mean of V.  Returns (lo, hi, info) as :func:`attn_interval`."""
+    L, dev = q.shape[0], q.device
+    d = q.shape[1] // heads
+    bf = torch.bfloat16
+    idx = torch.arange(L, device=dev)
+    off = idx[None, :] - idx[:, None] + (L - 1)
+    km = torch.ones(L, dtype=torch.bool, device=dev) if key_mask is None else key_mask.to(dev) != 0
+    us_lo, us_hi = [], []
+    for h in range(heads):
+        cs = slice(h * d, (h + 1) * d)
+        qh, kh, vh = q[:, cs].double(), k[:, cs].double(), v[:, cs].double()
+        S = qh @ kh.t()
+        E = c_s * (qh.abs() @ kh.abs().t())
+        b = bias_delta[h].double()[off]
+        val_lo = torch.where(km[None], r16(r16(S - E, bf) + b, bf), torch.full_like(S, T5_MIN))
+        val_hi = torch.where(km[None], r16(r16(S + E, bf) + b, bf), torch.full_like(S, T5_MIN))
+        m_lo = torch.full((L,), -float("inf"), dtype=F64, device=dev)
+        m_hi = m_lo.clone()
+        O_lo = torch.zeros(L, d, dtype=F64, device=dev)
+        O_hi, A = O_lo.clone(), O_lo.clone()
+        l_lo = torch.zeros(L, dtype=F64, device=dev)
+        l_hi = l_lo.clone()
+        n_tiles = (L + ATTN_TILE - 1) // ATTN_TILE
+        for k0 in range(0, L, ATTN_TILE):
+            k1 = min(k0 + ATTN_TILE, L)
+            vl, vu = val_lo[:, k0:k1], val_hi[:, k0:k1]
+            n_lo, n_hi = torch.maximum(m_lo, vl.amax(1)), torch.maximum(m_hi, vu.amax(1))
+            if k0 > 0:
+                a_lo, a_hi = (m_lo - n_hi) * LOG2E_F32, (m_hi - n_lo) * LOG2E_F32
+                al_lo, al_hi = _exp2_bounds(a_lo - 2 * U32 * a_lo.abs(), a_hi + 2 * U32 * a_hi.abs(), c_exp)
+                O_lo, O_hi = _scale_interval(O_lo, O_hi, al_lo[:, None], al_hi[:, None])
+                A = A * al_hi[:, None] * (1 + U32)
+                l_lo, l_hi = l_lo * al_lo, l_hi * al_hi
+            m_lo, m_hi = n_lo, n_hi
+            x_lo = (vl - m_hi[:, None]) * LOG2E_F32
+            x_hi = (vu - m_lo[:, None]) * LOG2E_F32
+            x_lo, x_hi = x_lo - 2 * U32 * x_lo.abs(), x_hi + 2 * U32 * x_hi.abs()
+            p_lo, p_hi = _exp2_bounds(x_lo, x_hi, c_exp)
+            P_lo, P_hi = r16(p_lo, bf), r16(p_hi, bf)
+            l_lo, l_hi = l_lo + p_lo.sum(1), l_hi + p_hi.sum(1)
+            a, b2, c = _pv_interval(P_lo, P_hi, vh[k0:k1])
+            O_lo, O_hi, A = O_lo + a, O_hi + b2, A + c
+        g = _l_chain(n_tiles, n_tiles)
+        l_lo, l_hi = l_lo * (1 - g), l_hi * (1 + g)
+        Eo = c_pv * A + 2.0 ** -120
+        inv_lo, inv_hi = (1 - U32) / l_hi, (1 + U32) / l_lo
+        lo, hi = _scale_interval(O_lo - Eo, O_hi + Eo, inv_lo[:, None], inv_hi[:, None])
+        us_lo.append(lo)
+        us_hi.append(hi)
+    u_lo, u_hi = torch.cat(us_lo, 1), torch.cat(us_hi, 1)
+    return r16(u_lo, bf), r16(u_hi, bf), {"u_lo": u_lo, "u_hi": u_hi, "ambiguous": 0, "heads": list(range(heads))}
+
+
+def check_attn(got, lo, hi, dtype, info=None):
+    """Hold an attention output to its restated interval with zero slack.  Returns (violations, stats): ``span``
+    (fraction of elements whose interval holds more than one 16-bit value), ``frac`` (fraction not equal to r16 of the
+    unrounded midpoint), ``ratio`` (the largest share of the interval's unrounded half-width an element needed: the
+    distance from the midpoint to the rounding boundary on the element's side, as :func:`acc_ratio`; <= 1 inside),
+    ``ambiguous`` (lazy decisions within the threshold's error margin)."""
+    viol = []
+    g = got.double()
+    if not bool(torch.isfinite(g).all()):
+        viol.append(f"{int((~torch.isfinite(g)).sum())} non-finite elements")
+        g = torch.nan_to_num(g, nan=1e300)
+    out = (g < lo) | (g > hi)
+    if bool(out.any()):
+        i = int(out.flatten().nonzero()[0])
+        r, c = divmod(i, g.shape[1])
+        viol.append(f"{int(out.sum())} elements outside the restated interval, first ({r}, {c}): "
+                    f"{float(g[r, c]):.8g} not in [{float(lo[r, c]):.8g}, {float(hi[r, c]):.8g}]")
+    stats = {"span": float((lo != hi).double().mean()), "ambiguous": 0, "ratio": 0.0, "frac": 0.0}
+    if info is not None:
+        mid = 0.5 * (info["u_lo"] + info["u_hi"])
+        half = 0.5 * (info["u_hi"] - info["u_lo"])
+        off = g != r16(mid, dtype)
+        stats["frac"] = float(off.double().mean())
+        stats["ambiguous"] = info["ambiguous"]
+        if bool(off.any()):
+            y, mm, hh = g[off], mid[off], half[off]
+            bnd = 0.5 * (y + _bits_neighbour(y, y < mm, dtype))
+            stats["ratio"] = float(((bnd - mm).abs() / hh.clamp_min(1e-300)).max())
+    return viol, stats
+
+
+# ---------------------------------------------------------------------------------------------
 # kr_vae.cu
 # ---------------------------------------------------------------------------------------------
 def vae_rmsnorm(x, gamma, dtype):

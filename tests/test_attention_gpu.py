@@ -12,7 +12,8 @@ Floating point, 16-bit inputs: P is rounded to 16 bits before P V, like FlashAtt
 store.  Tolerances: rel-L2 over the whole output <= 1e-2 (observed ~2.3e-3), and the relative L2 error of every
 (row, head) 128-vector <= 8e-3 (measured max on an H100: 4.0e-3; the bound keeps a 2x margin), so one wrong head of
 one row, an off-by-one in the padded-key count or at the window's lower edge fails.  Exact invariances (views, head
-slices, masks that hide nothing) are checked with ``torch.equal``."""
+slices, masks that hide nothing) are checked with ``torch.equal``.  These checks hold for any correct schedule; the
+element-wise check against a restatement of this kernel's own schedule is tests/test_attn_parity_gpu.py."""
 import math
 
 import pytest

@@ -1,6 +1,7 @@
 """GPU parity of the UMT5 encoder schedule (realtime_video_b200/t5.py through the C ABI, bf16 like the server runs it)
 against the reference T5Encoder goldens.  Tolerance: the reference's own bf16-vs-fp32 gap on this model is
-rel-L2 7e-3 (tests/golden/make_t5_goldens.py); we require <= 2e-2 against both goldens.
+rel-L2 7e-3 (tests/golden/make_t5_goldens.py); we require <= 2e-2 against both goldens.  The attention kernel alone
+(kr_t5_attn) is held element by element to a restatement of its schedule in tests/test_attn_parity_gpu.py.
 """
 import pytest
 import torch
@@ -22,42 +23,6 @@ def test_t5_encoder_vs_reference_golden(tag):
     for ref in ("fp32", "bf16"):
         r = rel_l2(y.float().cpu(), g[f"{tag}/{ref}"])
         assert r < 2e-2, f"{tag} vs {ref}: rel_l2={r:.3e}"
-
-
-def _t5_attn_ref(q, k, v, bias_delta, key_mask, heads):
-    """fp32 restatement with the reference's bf16 rounding points (wan/modules/t5.py:108-112)."""
-    L, d = q.shape[0], q.shape[1] // heads
-    qf = q.float().view(L, heads, d).transpose(0, 1)
-    kf = k.float().view(L, heads, d).transpose(0, 1)
-    vf = v.float().view(L, heads, d).transpose(0, 1)
-    off = torch.arange(L, device=q.device)[None, :] - torch.arange(L, device=q.device)[:, None] + (L - 1)
-    s = (qf @ kf.transpose(1, 2)).bfloat16()
-    bias = bias_delta[:, off]                                   # [heads, L, L] bf16
-    if key_mask is not None:
-        bias = bias.masked_fill(key_mask[None, None, :] == 0, torch.finfo(torch.bfloat16).min)
-    a = torch.softmax((s + bias).float(), dim=-1).bfloat16()
-    return (a.float() @ vf).transpose(0, 1).reshape(L, heads * d)
-
-
-@pytest.mark.parametrize("L,heads,valid", [(512, 64, 512), (512, 64, 37), (200, 4, 150), (128, 2, 128), (777, 3, 700)])
-def test_t5_attention_kernel_vs_fp32_reference(L, heads, valid):
-    """kr_t5_attn (head_dim 64, bias by offset, key mask) at the UMT5-XXL shape (L 512, 64 heads) and ragged ones
-    (L not a multiple of the 128-row / 256-key tiles, 3 key tiles).  P is rounded un-normalised: rel-L2 <= 1e-2."""
-    from realtime_video_b200 import ops
-    torch.manual_seed(L + heads)
-    D = heads * 64
-    q = (torch.randn(L, D, device="cuda") * 0.6).bfloat16()
-    k = (torch.randn(L, D, device="cuda") * 0.6).bfloat16()
-    v = torch.randn(L, D, device="cuda").bfloat16()
-    bias = (torch.randn(heads, 2 * L - 1, device="cuda") * 2).bfloat16()
-    km = None
-    if valid < L:
-        km = torch.zeros(L, dtype=torch.uint8, device="cuda")
-        km[:valid] = 1
-    out = ops.t5_attention(q, k, v, bias, km, heads=heads)
-    ref = _t5_attn_ref(q, k, v, bias, km, heads)
-    r = rel_l2(out.float(), ref)
-    assert torch.isfinite(out).all() and r < 1e-2, r
 
 
 def test_umt5_xxl_dims_two_layers_vs_oracle():
