@@ -325,5 +325,8 @@ int kr_rgb8_to_jpeg(const unsigned char* rgb, int frames, int height, int width,
 /* The FP8 tier of the VAE decoder's convolutions (kr_vae_conv_fp8 / kr_vae_rmsnorm_silu_fp8): likewise its own header;
  * the entry points live with the kernels in kr_vae.cu. */
 #include "krea_b200_vae_fp8.h"
+/* Block-scaled FP8 linears (kr_fp8_quantize_blocks / kr_ln_modulate_fp8_blocks / kr_gemm_fp8_blockwise): a header of
+ * their own beside the PerTensor / PerRow entry points above; the API layer kr_api.cu defines them. */
+#include "krea_b200_fp8_blocks.h"
 
 #endif /* KREA_B200_H_ */

@@ -177,6 +177,15 @@ VAE_FP8_SIGNATURES = {
 }
 VAE_FP8_SIGNATURES["kr_vae_conv_fp8_sub2"] = VAE_FP8_SIGNATURES["kr_vae_conv_fp8"]
 
+# the block-scaled FP8 linears (include/krea_b200_fp8_blocks.h, kr_dit_elem.cu / kr_gemm_fp8.cu); every function returns int
+FP8_BLOCK_SIGNATURES = {
+    "kr_fp8_quantize_blocks": [_vp, _i, _i, _i, _vp, _i, _vp, _i, _vp],
+    "kr_ln_modulate_fp8_blocks": [_vp, _i, _vp, _i, _i, _i, _f, _vp, _vp, _vp, _i, _i, _i, _i, _i, _vp, _i, _vp, _i,
+                                  _vp],
+    "kr_gemm_fp8_blockwise": [_i, _vp, _i, _vp, _i, _vp, _i, _vp, _vp, _vp, _i, _i, _i, _i, _vp, _i, _vp, _i, _i, _vp,
+                              _i, _i, _i, _vp],
+}
+
 
 def load() -> ctypes.CDLL:
     """Load the shared library (building is the caller's job: ``__graft_entry__.build``)."""
@@ -203,7 +212,7 @@ def load() -> ctypes.CDLL:
         if hasattr(lib, "kr_jpeg_workspace_bytes"):
             lib.kr_jpeg_workspace_bytes.restype = _sz
             lib.kr_jpeg_workspace_bytes.argtypes = [_i, _i, _i]
-        for name, argtypes in {**SIGNATURES, **SAGE_SIGNATURES, **VAE_FP8_SIGNATURES}.items():
+        for name, argtypes in {**SIGNATURES, **SAGE_SIGNATURES, **VAE_FP8_SIGNATURES, **FP8_BLOCK_SIGNATURES}.items():
             fn = getattr(lib, name, None)
             if fn is None:
                 continue   # checked by tests/test_abi.py against the header

@@ -148,6 +148,47 @@ int kr_gemm_fp8_rowwise_fast(int epilogue, const void* a, int lda, const void* w
                                       static_cast<cudaStream_t>(stream));
 }
 
+// Block-scaled FP8 (include/krea_b200_fp8_blocks.h): shapes the kernels cannot run are argument errors, reported
+// before anything touches the device.
+int kr_fp8_quantize_blocks(const void* x, int ldx, int rows, int cols, void* q, int ldq, float* scale, int ld_s,
+                           void* stream) {
+  KR_REQUIRE(x && q && scale, "null x/q/scale");
+  KR_REQUIRE(rows > 0 && cols > 0 && cols % 128 == 0 && ld_s >= rows, "need cols % 128 == 0 and ld_s >= rows");
+  KR_REQUIRE_LINKED(fp8_quantize_blocks);
+  return kr::fp8_quantize_blocks(x, ldx, rows, cols, q, ldq, scale, ld_s, static_cast<cudaStream_t>(stream));
+}
+
+int kr_ln_modulate_fp8_blocks(const void* x, int ldx, void* out, int ldo, int rows, int D, float eps,
+                              const void* w, const void* b, const void* mod, int mod_rows, int shift_idx,
+                              int scale_idx, int rows_per_frame, int row_offset, void* q, int ldq, float* scale,
+                              int ld_s, void* stream) {
+  KR_REQUIRE(x && q && scale, "null x/q/scale");
+  KR_REQUIRE(rows > 0 && D > 0 && D % 128 == 0 && ld_s >= rows, "need D % 128 == 0 and ld_s >= rows");
+  KR_REQUIRE_LINKED(ln_modulate_fp8_blocks);
+  return kr::ln_modulate_fp8_blocks(x, ldx, out, ldo, rows, D, eps, w, b, mod, mod_rows, shift_idx, scale_idx,
+                                    rows_per_frame, row_offset, q, ldq, scale, ld_s,
+                                    static_cast<cudaStream_t>(stream));
+}
+
+int kr_gemm_fp8_blockwise(int epilogue, const void* a, int lda, const void* w, int ldw, const float* scale_a,
+                          int ld_sa, const float* scale_w, const void* bias, void* out, int ldc, int M, int N, int K,
+                          const void* residual, int ldr, const void* gate, int gate_stride, int rows_per_gate,
+                          void* out2, int ldc2, int n_split, int row_offset, void* stream) {
+  KR_REQUIRE(a && w && out, "null a/w/out");
+  KR_REQUIRE(scale_a && scale_w, "null scale_a/scale_w");
+  KR_REQUIRE(M > 0 && N > 0 && K > 0 && N % 128 == 0 && K % 128 == 0, "need N % 128 == 0 and K % 128 == 0");
+  KR_REQUIRE(lda % 16 == 0 && ldw % 16 == 0 && lda >= K && ldw >= K && ldc % 8 == 0 && ldc > 0 && ld_sa >= M,
+             "pitches: lda / ldw >= K and % 16 == 0, ldc % 8 == 0, ld_sa >= M");
+  KR_REQUIRE_LINKED(gemm_fp8_blockwise_tn);
+  kr::GemmParams p;
+  p.out = out; p.bias = bias; p.residual = residual; p.gate = gate;
+  p.M = M; p.N = N; p.K = K; p.ldc = ldc; p.ldr = ldr; p.gate_stride = gate_stride;
+  p.rows_per_gate = rows_per_gate; p.alpha = 1.0f;
+  p.out2 = out2; p.ldc2 = ldc2; p.n_split = n_split; p.row_offset = row_offset;
+  return kr::gemm_fp8_blockwise_tn(epilogue, a, lda, w, ldw, p, scale_a, ld_sa, scale_w,
+                                   static_cast<cudaStream_t>(stream));
+}
+
 int kr_attn_fwd(int dtype, const void* q, int ldq, const void* k, int ldk, const void* v, int ldv,
                 void* out, int ldo, int Lq, int Lkv, int heads, float softmax_scale, int mask_mode,
                 int block_len, int window, int pad_keys, void* stream) {

@@ -115,12 +115,53 @@ KR_DEVICE void fp8_quantize_row(const uint4 (&raw)[kVec], int nvec, float* red, 
   }
 }
 
-template <int kVec, bool kFp8>
+// Dynamic e4m3 cast of one row per 128-channel group (torchao PerBlock [1, 128]), the row held packed in registers by
+// a kRowThreads CTA: a group is 16 consecutive 8-channel vectors, i.e. the vectors i of 16 consecutive lanes, so its
+// amax is a 16-lane shuffle reduction (no shared memory, no barrier).  Per group g:
+//   amax = max(max|x_g|, 1e-12), q_g = sat_e4m3(x_g * (448 / amax)), scale_col[g * ld_s] = amax / 448.
+// nvec must be a multiple of 16 (cols % 128 == 0), so a group is either wholly valid or wholly past the row's end.
+template <int kVec>
+KR_DEVICE void fp8_quantize_row_groups(const uint4 (&raw)[kVec], int nvec, uint8_t* __restrict__ qrow,
+                                       float* __restrict__ scale_col, int ld_s) {
+#pragma unroll
+  for (int i = 0; i < kVec; ++i) {
+    const int vi = threadIdx.x + i * kRowThreads;
+    const bool valid = vi < nvec;
+    const uint32_t u[4] = {raw[i].x, raw[i].y, raw[i].z, raw[i].w};
+    float m = 0.f;
+    if (valid) {
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        const float2 f = unpack_bf16x2(u[j]);
+        m = fmaxf(m, fmaxf(fabsf(f.x), fabsf(f.y)));
+      }
+    }
+#pragma unroll
+    for (int o = 8; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));   // all lanes take part
+    if (valid) {
+      const float amax = fmaxf(m, 1e-12f);
+      const float mul = 448.0f / amax;
+      if ((threadIdx.x & 15) == 0) scale_col[static_cast<size_t>(vi >> 4) * ld_s] = amax / 448.0f;
+      uint32_t o[2];
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        const float2 f = unpack_bf16x2(u[j]);
+        const uint32_t h = __nv_cvt_float2_to_fp8x2(make_float2(f.x * mul, f.y * mul), __NV_SATFINITE, __NV_E4M3);
+        if (j & 1) o[j >> 1] |= h << 16;
+        else o[j >> 1] = h;
+      }
+      *reinterpret_cast<uint2*>(qrow + vi * 8) = make_uint2(o[0], o[1]);
+    }
+  }
+}
+
+// kBlocks (with kFp8): the cast is per 128-channel group (fp8_quantize_row_groups) into q / scale_rows[g * ld_s].
+template <int kVec, bool kFp8, bool kBlocks = false>
 KR_DEVICE void ln_modulate_row(const uint16_t* __restrict__ x, int ldx, uint16_t* __restrict__ out, int ldo,
                                int D, float eps, const uint16_t* __restrict__ w, const uint16_t* __restrict__ b,
                                const uint16_t* __restrict__ mod, int mod_rows, int shift_idx, int scale_idx,
                                int rows_per_frame, int row_offset, uint8_t* __restrict__ q, int ldq,
-                               float* __restrict__ scale_rows) {
+                               float* __restrict__ scale_rows, int ld_s = 0) {
   __shared__ float red[4];
   const int row = blockIdx.x;
   const uint16_t* xr = x + static_cast<size_t>(row) * ldx;
@@ -194,7 +235,10 @@ KR_DEVICE void ln_modulate_row(const uint16_t* __restrict__ x, int ldx, uint16_t
       }
     }
   }
-  if constexpr (kFp8) fp8_quantize_row<kVec>(raw, nvec, red, q + static_cast<size_t>(row) * ldq, scale_rows + row);
+  if constexpr (kFp8 && kBlocks)
+    fp8_quantize_row_groups<kVec>(raw, nvec, q + static_cast<size_t>(row) * ldq, scale_rows + row, ld_s);
+  else if constexpr (kFp8)
+    fp8_quantize_row<kVec>(raw, nvec, red, q + static_cast<size_t>(row) * ldq, scale_rows + row);
 }
 
 template <int kVec>
@@ -216,6 +260,17 @@ ln_modulate_fp8_kernel(const uint16_t* __restrict__ x, int ldx, uint16_t* __rest
                        float* __restrict__ scale_rows) {
   ln_modulate_row<kVec, true>(x, ldx, out, ldo, D, eps, w, b, mod, mod_rows, shift_idx, scale_idx, rows_per_frame,
                               row_offset, q, ldq, scale_rows);
+}
+
+template <int kVec>
+__global__ void __launch_bounds__(kRowThreads, 8)
+ln_modulate_fp8_blocks_kernel(const uint16_t* __restrict__ x, int ldx, uint16_t* __restrict__ out, int ldo,
+                              int D, float eps, const uint16_t* __restrict__ w, const uint16_t* __restrict__ b,
+                              const uint16_t* __restrict__ mod, int mod_rows, int shift_idx, int scale_idx,
+                              int rows_per_frame, int row_offset, uint8_t* __restrict__ q, int ldq,
+                              float* __restrict__ scale, int ld_s) {
+  ln_modulate_row<kVec, true, true>(x, ldx, out, ldo, D, eps, w, b, mod, mod_rows, shift_idx, scale_idx,
+                                    rows_per_frame, row_offset, q, ldq, scale, ld_s);
 }
 
 static int ln_check(const char* who, int rows, int D, int ldx, int ldo, const void* w, const void* b, const void* mod,
@@ -296,6 +351,37 @@ int ln_modulate_fp8(const void* x, int ldx, void* out, int ldo, int rows, int D,
   return launch_status("ln_modulate_fp8");
 }
 
+int ln_modulate_fp8_blocks(const void* x, int ldx, void* out, int ldo, int rows, int D, float eps,
+                           const void* w, const void* b, const void* mod, int mod_rows, int shift_idx,
+                           int scale_idx, int rows_per_frame, int row_offset, void* q, int ldq, float* scale,
+                           int ld_s, cudaStream_t stream) {
+  const int rc = ln_check("ln_modulate_fp8_blocks", rows, D, ldx, out != nullptr ? ldo : 8, w, b, mod,
+                          rows_per_frame);
+  if (rc != KR_OK) return rc;
+  if (D % 128 != 0 || ldq % 16 != 0 || ldq < D || ld_s < rows) {
+    set_last_error("ln_modulate_fp8_blocks: unsupported D=%d ldq=%d ld_s=%d rows=%d (need D %% 128 == 0)", D, ldq,
+                   ld_s, rows);
+    return KR_ERR_UNSUPPORTED_SHAPE;
+  }
+  const int nv = (D / 8 + kRowThreads - 1) / kRowThreads;
+#define KR_LN_LAUNCH(V)                                                                            \
+  ln_modulate_fp8_blocks_kernel<V><<<rows, kRowThreads, 0, stream>>>(                              \
+      static_cast<const uint16_t*>(x), ldx, static_cast<uint16_t*>(out), ldo, D, eps,              \
+      static_cast<const uint16_t*>(w), static_cast<const uint16_t*>(b),                            \
+      static_cast<const uint16_t*>(mod), mod_rows, shift_idx, scale_idx, rows_per_frame, row_offset, \
+      static_cast<uint8_t*>(q), ldq, scale, ld_s)
+  switch (nv) {
+    case 1: KR_LN_LAUNCH(1); break;
+    case 2: KR_LN_LAUNCH(2); break;
+    case 3: KR_LN_LAUNCH(3); break;
+    case 4: KR_LN_LAUNCH(4); break;
+    case 5: KR_LN_LAUNCH(5); break;
+    default: KR_LN_LAUNCH(8); break;
+  }
+#undef KR_LN_LAUNCH
+  return launch_status("ln_modulate_fp8_blocks");
+}
+
 // ---------------------------------------------------------------------------
 // Dynamic per-row e4m3 activation cast (torchao Float8DynamicActivation, PerRow): one CTA per row, the row in
 // registers, one read and one write; scale_rows[r] = amax_r / 448 is the row scale of the row-scaled FP8 GEMM.
@@ -344,6 +430,52 @@ int fp8_quantize_rows(const void* x, int ldx, int rows, int cols, void* q, int l
   }
 #undef KR_Q_LAUNCH
   return launch_status("fp8_quantize_rows");
+}
+
+// Dynamic per-group e4m3 activation cast (torchao PerBlock [1, 128]): the row quantiser's CTA-per-row layout, one
+// scale per 128-channel group stored k-block-major (scale[g * ld_s + r]: one k-block's row scales are contiguous for
+// the block-scaled GEMM).  One read, one write, no atomics, no memset.
+template <int kVec>
+__global__ void __launch_bounds__(kRowThreads)
+fp8_quantize_blocks_kernel(const uint16_t* __restrict__ x, int ldx, int cols, uint8_t* __restrict__ q, int ldq,
+                           float* __restrict__ scale, int ld_s) {
+  const int row = blockIdx.x;
+  const uint16_t* xr = x + static_cast<size_t>(row) * ldx;
+  const int nvec = cols >> 3;
+  uint4 raw[kVec];
+#pragma unroll
+  for (int i = 0; i < kVec; ++i) {
+    const int vi = threadIdx.x + i * kRowThreads;
+    if (vi < nvec) raw[i] = *reinterpret_cast<const uint4*>(xr + vi * 8);
+  }
+  fp8_quantize_row_groups<kVec>(raw, nvec, q + static_cast<size_t>(row) * ldq, scale + row, ld_s);
+}
+
+int fp8_quantize_blocks(const void* x, int ldx, int rows, int cols, void* q, int ldq, float* scale, int ld_s,
+                        cudaStream_t stream) {
+  if (cols <= 0 || cols % 128 != 0 || cols > kRowThreads * 8 * kQuantMaxVec || rows <= 0 || ldx % 8 != 0 ||
+      ldq % 16 != 0 || ldx < cols || ldq < cols || ld_s < rows) {
+    set_last_error("fp8_quantize_blocks: unsupported rows=%d cols=%d ldx=%d ldq=%d ld_s=%d", rows, cols, ldx, ldq,
+                   ld_s);
+    return KR_ERR_UNSUPPORTED_SHAPE;
+  }
+  const int nv = (cols / 8 + kRowThreads - 1) / kRowThreads;
+#define KR_Q_LAUNCH(V)                                                                             \
+  fp8_quantize_blocks_kernel<V><<<rows, kRowThreads, 0, stream>>>(                                 \
+      static_cast<const uint16_t*>(x), ldx, cols, static_cast<uint8_t*>(q), ldq, scale, ld_s)
+  switch (nv) {
+    case 1: KR_Q_LAUNCH(1); break;
+    case 2: KR_Q_LAUNCH(2); break;
+    case 3: KR_Q_LAUNCH(3); break;
+    case 4: KR_Q_LAUNCH(4); break;
+    case 5: KR_Q_LAUNCH(5); break;
+    case 6: KR_Q_LAUNCH(6); break;
+    case 7: case 8: KR_Q_LAUNCH(8); break;
+    case 9: case 10: KR_Q_LAUNCH(10); break;
+    default: KR_Q_LAUNCH(14); break;
+  }
+#undef KR_Q_LAUNCH
+  return launch_status("fp8_quantize_blocks");
 }
 
 // ---------------------------------------------------------------------------

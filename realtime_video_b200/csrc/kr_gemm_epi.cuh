@@ -187,7 +187,60 @@ KR_DEVICE void gemm_mainloop(float (&acc)[BN / 2], uint32_t a_base, uint32_t b_b
   if (prev >= 0 && leader) release_stage<kCluster>(&empty[prev]);
 }
 
-constexpr int kEpiScrPitch = 36;                       // floats per scratch row (16-byte aligned, fewer conflicts)
+// Per-k-block dequantisation scales of the block-scaled FP8 GEMM, as one consumer thread sees them: the activation
+// scales of its two accumulator rows (row and row + 8 of its warp's 16) at k-block 0 with k-block pitch `ld` (null
+// for a row >= M: it reads no scale), and the tile's weight-block scales, one per k-block.
+struct BlockScales {
+  const float* __restrict__ sa0;
+  const float* __restrict__ sa1;
+  long ld;
+  const float* __restrict__ sw;
+};
+
+// The block-scaled accumulation mode of gemm_mainloop (kBlockScale, promoted e4m3 only): each k-block's partial is
+// multiplied by its row's activation scale times the tile's weight scale before the fp32 add
+// (acc += part * sa[kb][row] * sw[kb]).  The scales of k-block kb + 1 are loaded while kb's wgmma runs, so the loop
+// waits on nothing new.  An overload rather than a branch of the function above: a block-scale argument added to that
+// function changed the machine code of the kernels that do not use it.
+template <int BN, int kKind, int kCluster, bool kPromote, bool kBlockScale>
+KR_DEVICE void gemm_mainloop(float (&acc)[BN / 2], uint32_t a_base, uint32_t b_base, int a_bytes, int b_bytes,
+                             int stages, uint64_t* full, uint64_t* empty, int& stage, uint32_t& phase, int kb0,
+                             int kb1, const BlockScales& bs) {
+  static_assert(kKind == 2 && kPromote && kBlockScale, "block scales are applied at the e4m3 promotion");
+  const bool leader = (threadIdx.x & 127) == 0;
+  float part[BN / 2];
+  float na0 = bs.sa0 != nullptr ? __ldg(bs.sa0 + kb0 * bs.ld) : 0.f;
+  float na1 = bs.sa1 != nullptr ? __ldg(bs.sa1 + kb0 * bs.ld) : 0.f;
+  float nw = __ldg(bs.sw + kb0);
+  for (int kb = kb0; kb < kb1; ++kb) {
+    const float s0 = na0 * nw, s1 = na1 * nw;
+    if (kb + 1 < kb1) {
+      if (bs.sa0 != nullptr) na0 = __ldg(bs.sa0 + (kb + 1) * bs.ld);
+      if (bs.sa1 != nullptr) na1 = __ldg(bs.sa1 + (kb + 1) * bs.ld);
+      nw = __ldg(bs.sw + kb + 1);
+    }
+    mbar_wait(&full[stage], phase);
+    const uint32_t a = a_base + stage * a_bytes, b = b_base + stage * b_bytes;
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < 4; ++k)
+      gemm_k_step<BN, kKind>(part, make_smem_desc(a + k * 32, 16, 1024), make_smem_desc(b + k * 32, 16, 1024),
+                             k != 0 ? 1 : 0);
+    wgmma_commit();
+    wgmma_wait<0>();
+    reg_fence(part);
+    if (leader) release_stage<kCluster>(&empty[stage]);
+    // fragment layout of m64nNk32: elements 4j, 4j + 1 belong to the thread's first row, 4j + 2, 4j + 3 to row + 8
+#pragma unroll
+    for (int i = 0; i < BN / 2; ++i) acc[i] = (kb == kb0 ? 0.f : acc[i]) + part[i] * ((i & 2) ? s1 : s0);
+    if (++stage == stages) {
+      stage = 0;
+      phase ^= 1;
+    }
+  }
+}
+
+constexpr int kEpiScrPitch = 36;                      // floats per scratch row (16-byte aligned, fewer conflicts)
 constexpr int kEpiScrFloats = 16 * kEpiScrPitch;       // one warp's 16 x 32 transpose buffer
 
 // The fragment of one warp (rows row0 .. row0+15 of the output, columns col_base + [0, BN)) -> fused epilogue.

@@ -1,8 +1,9 @@
-// kr_gemm_fp8.cu — FP8 (e4m3) wgmma GEMM with per-tensor or per-row scales + the dynamic per-tensor activation
+// kr_gemm_fp8.cu — FP8 (e4m3) wgmma GEMM with per-tensor, per-row or per-block scales + the dynamic per-tensor activation
 // quantisation kernels (the per-row quantiser lives with the row kernels in kr_dit_elem.cu).
 //
 //   per tensor: out[M,N] = epilogue( (Aq[M,K] @ Wq[N,K]^T) * scale_a * scale_w + bias[N] )    Aq, Wq e4m3, out bf16
 //   per row   : out[M,N] = epilogue( (Aq[M,K] @ Wq[N,K]^T) * scale_a[m] * scale_w[n] + bias[N] )
+//   per block : out[M,N] = epilogue( sum_kb (Aq[M,kb] @ Wq[N,kb]^T) * scale_a[kb][m] * scale_w[n/128][kb] + bias[N] )
 //
 // Replaces, on the reference path, what `quantize_(transformer, Float8DynamicActivationFloat8WeightConfig(
 // granularity=PerTensor()))` (release_server.py:179-182, `enable_fp8: true`) turns every nn.Linear into: torchao's
@@ -199,6 +200,84 @@ gemm_fp8_fast_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_co
   }
 }
 
+// Block scaling (torchao PerBlock [1, 128] activations / [128, 128] weights, the DeepSeek-V3 recipe): the promoted
+// kernel's structure and tile, with each k-block's partial multiplied by sa[kb][row] * sw[n_blk][kb] at the promotion
+// (gemm_mainloop<..., kBlockScale>).  The 128 x 128 tile spans exactly one weight block in N and one activation group
+// per k-block, so the epilogue applies no scale.  A kernel of its own for the reason given above the fast kernel.
+//   scale_a: fp32 [K/128, ld_sa] (k-block-major: one k-block's row scales are contiguous), scale_w: fp32 [N/128, K/128]
+template <int kEpi>
+__global__ void __launch_bounds__(F8_THREADS, 1)
+gemm_fp8_blockwise_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
+                          const GemmParams p, const float* __restrict__ scale_a, long ld_sa,
+                          const float* __restrict__ scale_w) {
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
+                                             ~static_cast<uintptr_t>(1023));
+  uint8_t* smem_a = smem;
+  uint8_t* smem_b = smem + F8_STAGES * F8_A_BYTES;
+  float* scratch = reinterpret_cast<float*>(smem + F8_STAGES * F8_STAGE_BYTES);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + F8_STAGES * F8_STAGE_BYTES + F8_SCR_BYTES);
+  uint64_t* full_bar = bars;
+  uint64_t* empty_bar = bars + F8_STAGES;
+
+  const int warp = threadIdx.x >> 5;
+  const int num_m = (p.M + F8_BM - 1) / F8_BM, num_n = p.N / F8_BN, num_tiles = num_m * num_n;
+  const int num_k = (p.K + F8_BK - 1) / F8_BK;
+
+  if (threadIdx.x == 256) {
+    prefetch_tmap(&tmap_a);
+    prefetch_tmap(&tmap_b);
+    for (int i = 0; i < F8_STAGES; ++i) {
+      mbar_init(&full_bar[i], 1);
+      mbar_init(&empty_bar[i], 2);
+    }
+    fence_barrier_init();
+  }
+  __syncthreads();
+
+  if (warp >= 8) {
+    producer_regs();
+    if (warp == 8 && elect_one()) {
+      int stage = 0;
+      uint32_t phase = 0;
+      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+        const int m_blk = tile % num_m, n_blk = tile / num_m;
+        for (int kb = 0; kb < num_k; ++kb) {
+          mbar_wait(&empty_bar[stage], phase ^ 1);
+          mbar_expect_tx(&full_bar[stage], F8_STAGE_BYTES);
+          tma_load_2d(smem_a + stage * F8_A_BYTES, &tmap_a, &full_bar[stage], kb * F8_BK, m_blk * F8_BM);
+          tma_load_2d(smem_b + stage * F8_B_BYTES, &tmap_b, &full_bar[stage], kb * F8_BK, n_blk * F8_BN);
+          if (++stage == F8_STAGES) {
+            stage = 0;
+            phase ^= 1;
+          }
+        }
+      }
+    }
+    return;
+  }
+  consumer_regs();
+  const int wg = warp >> 2, lane = threadIdx.x & 31;
+  const uint32_t a_base = smem_u32(smem_a) + wg * 64 * F8_BK, b_base = smem_u32(smem_b);
+  float* scr = scratch + warp * kEpiScrFloats;
+  int stage = 0;
+  uint32_t phase = 0;
+  for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+    const int m_blk = tile % num_m, n_blk = tile / num_m;
+    const int row0 = m_blk * F8_BM + wg * 64 + (warp & 3) * 16;
+    const int r = row0 + (lane >> 2);
+    BlockScales bs;
+    bs.sa0 = r < p.M ? scale_a + r : nullptr;
+    bs.sa1 = r + 8 < p.M ? scale_a + r + 8 : nullptr;
+    bs.ld = ld_sa;
+    bs.sw = scale_w + static_cast<long>(n_blk) * num_k;
+    float acc[F8_BN / 2];
+    gemm_mainloop<F8_BN, 2, 1, true, true>(acc, a_base, b_base, F8_A_BYTES, F8_B_BYTES, F8_STAGES, full_bar,
+                                           empty_bar, stage, phase, 0, num_k, bs);
+    gemm_frag_epilogue<F8_BN, true, kEpi>(acc, scr, row0, n_blk * F8_BN, F8_BN, 1.f, p);
+  }
+}
+
 // ---------------------------------------------------------------------------
 // dynamic per-tensor activation quantisation: amax -> scale -> saturating e4m3 cast
 // ---------------------------------------------------------------------------
@@ -386,6 +465,67 @@ int gemm_fp8_fast_tn(int epi, const void* a, int lda, const void* w, int ldw, co
 int gemm_fp8_rowwise_fast_tn(int epi, const void* a, int lda, const void* w, int ldw, const GemmParams& p,
                              const float* scale_a, const float* scale_w, cudaStream_t stream) {
   return gemm_fp8_rowwise_any<true>("gemm_fp8_rowwise_fast", epi, a, lda, w, ldw, p, scale_a, scale_w, stream);
+}
+
+template <int kEpi>
+static int launch_fp8_blockwise(const void* a, int lda, const void* w, int ldw, const GemmParams& p,
+                                const float* scale_a, long ld_sa, const float* scale_w, cudaStream_t stream) {
+  CUtensorMap ta, tb;
+  const uint64_t da[2] = {static_cast<uint64_t>(p.K), static_cast<uint64_t>(p.M)};
+  const uint64_t sa[1] = {static_cast<uint64_t>(lda)};
+  const uint32_t ba[2] = {F8_BK, F8_BM};
+  int rc = make_tmap_u8(&ta, a, 2, da, sa, ba, 128);
+  if (rc != KR_OK) return rc;
+  const uint64_t db[2] = {static_cast<uint64_t>(p.K), static_cast<uint64_t>(p.N)};
+  const uint64_t sb[1] = {static_cast<uint64_t>(ldw)};
+  const uint32_t bb[2] = {F8_BK, F8_BN};
+  rc = make_tmap_u8(&tb, w, 2, db, sb, bb, 128);
+  if (rc != KR_OK) return rc;
+  static bool attr_set = false;
+  if (!attr_set) {
+    cudaError_t e = cudaFuncSetAttribute(gemm_fp8_blockwise_kernel<kEpi>,
+                                         cudaFuncAttributeMaxDynamicSharedMemorySize, F8_SMEM);
+    if (e != cudaSuccess) {
+      set_last_error("gemm_fp8_blockwise: cudaFuncSetAttribute failed: %s", cudaGetErrorString(e));
+      return KR_ERR_CUDA;
+    }
+    attr_set = true;
+  }
+  const int num_tiles = ((p.M + F8_BM - 1) / F8_BM) * (p.N / F8_BN);
+  int grid = sm_count();
+  if (grid > num_tiles) grid = num_tiles;
+  gemm_fp8_blockwise_kernel<kEpi><<<grid, F8_THREADS, F8_SMEM, stream>>>(ta, tb, p, scale_a, ld_sa, scale_w);
+  cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) {
+    set_last_error("gemm_fp8_blockwise: launch failed: %s", cudaGetErrorString(e));
+    return KR_ERR_CUDA;
+  }
+  return KR_OK;
+}
+
+int gemm_fp8_blockwise_tn(int epi, const void* a, int lda, const void* w, int ldw, const GemmParams& p,
+                          const float* scale_a, int ld_sa, const float* scale_w, cudaStream_t stream) {
+  // the host-side checks of kr_api.cu (shape, pitches, null scales) have passed; these guard direct callers
+  const char* who = "gemm_fp8_blockwise";
+  int rc = check_fp8(who, F8_BN, epi, lda, ldw, p);
+  if (rc != KR_OK) return rc;
+  if (p.K % F8_BK != 0) {
+    set_last_error("%s: K=%d is not a multiple of the 128-wide scale block", who, p.K);
+    return KR_ERR_UNSUPPORTED_SHAPE;
+  }
+  if (scale_a == nullptr || scale_w == nullptr || ld_sa < p.M) {
+    set_last_error("%s: null block scales or activation scale pitch %d < M=%d", who, ld_sa, p.M);
+    return KR_ERR_INVALID_ARG;
+  }
+  switch (epi) {
+    case EPI_BIAS: return launch_fp8_blockwise<EPI_BIAS>(a, lda, w, ldw, p, scale_a, ld_sa, scale_w, stream);
+    case EPI_BIAS_GELU: return launch_fp8_blockwise<EPI_BIAS_GELU>(a, lda, w, ldw, p, scale_a, ld_sa, scale_w, stream);
+    case EPI_BIAS_GATE_RES:
+      return launch_fp8_blockwise<EPI_BIAS_GATE_RES>(a, lda, w, ldw, p, scale_a, ld_sa, scale_w, stream);
+    case EPI_BIAS_RES: return launch_fp8_blockwise<EPI_BIAS_RES>(a, lda, w, ldw, p, scale_a, ld_sa, scale_w, stream);
+    case EPI_F32: return launch_fp8_blockwise<EPI_F32>(a, lda, w, ldw, p, scale_a, ld_sa, scale_w, stream);
+    default: set_last_error("%s: unsupported epilogue %d", who, epi); return KR_ERR_INVALID_ARG;
+  }
 }
 
 }  // namespace kr

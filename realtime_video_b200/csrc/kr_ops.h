@@ -68,6 +68,19 @@ __attribute__((weak)) int gemm_fp8_fast_tn(int epi, const void* a, int lda, cons
 __attribute__((weak)) int gemm_fp8_rowwise_fast_tn(int epi, const void* a, int lda, const void* w, int ldw,
                                                    const GemmParams& p, const float* scale_a, const float* scale_w,
                                                    cudaStream_t stream);
+// Block-scaled FP8 (torchao PerBlock [1, 128] / [128, 128]): the per-128-channel-group e4m3 cast and the LayerNorm
+// writing it (kr_dit_elem.cu; scales k-block-major [cols / 128, ld_s]), and the promoted FP8 GEMM applying
+// sa[kb][m] * sw[n / 128][kb] to each k-block's partial (kr_gemm_fp8.cu).  Weak for the same reason.
+__attribute__((weak)) int fp8_quantize_blocks(const void* x, int ldx, int rows, int cols, void* q, int ldq,
+                                              float* scale, int ld_s, cudaStream_t stream);
+__attribute__((weak)) int ln_modulate_fp8_blocks(const void* x, int ldx, void* out, int ldo, int rows, int D,
+                                                 float eps, const void* w, const void* b, const void* mod,
+                                                 int mod_rows, int shift_idx, int scale_idx, int rows_per_frame,
+                                                 int row_offset, void* q, int ldq, float* scale, int ld_s,
+                                                 cudaStream_t stream);
+__attribute__((weak)) int gemm_fp8_blockwise_tn(int epi, const void* a, int lda, const void* w, int ldw,
+                                                const GemmParams& p, const float* scale_a, int ld_sa,
+                                                const float* scale_w, cudaStream_t stream);
 // 2-CTA cluster variant (W multicast to both CTAs, 128x256 tile per CTA), kr_gemm2.cu; N % 256 == 0
 int gemm2_tn(int dtype, int epi, const void* a, int lda, const void* w, int ldw, const GemmParams& p,
              cudaStream_t stream);

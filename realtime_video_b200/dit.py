@@ -32,11 +32,14 @@ from . import fp8, ops
 def _linear(x, lin: nn.Linear, **kw) -> torch.Tensor:
     """nn.Linear of a DiT block on the GEMM kernels: bf16 by default, FP8 (dynamic activation cast + e4m3 wgmma GEMM)
     when ``realtime_video_b200.fp8.quantize_`` attached quantised weights to the module, with the granularity it
-    attached: per tensor, or per row (``x`` may then be an ``ops.Fp8Rows`` the LayerNorm already cast), and with the
-    accumulation mode it recorded (``fast_accum`` is passed only when chosen)."""
+    attached: per tensor, per row (``x`` may then be an ``ops.Fp8Rows`` the LayerNorm already cast) or per block (``x``
+    may be an ``ops.Fp8Blocks``), and with the accumulation mode it recorded (``fast_accum`` is passed only when
+    chosen; block scaling is promoted only)."""
     q = getattr(lin, "_kr_fp8", None)
     if q is None:
         return ops.gemm(x, lin.weight, lin.bias, **kw)
+    if fp8.is_blockwise(lin):
+        return ops.linear_fp8_blockwise(x, q[0], q[1], lin.bias, **kw)
     if fp8.is_fast_accum(lin):
         kw["fast_accum"] = True
     if fp8.is_rowwise(lin):
@@ -47,6 +50,22 @@ def _linear(x, lin: nn.Linear, **kw) -> torch.Tensor:
 def _rowwise(*lins: nn.Module) -> bool:
     """Every one of ``lins`` runs the PerRow FP8 GEMM: their common input can be cast to e4m3 once, by its producer."""
     return all(fp8.is_rowwise(m) for m in lins)
+
+
+def _blockwise(*lins: nn.Module) -> bool:
+    """Every one of ``lins`` runs the PerBlock FP8 GEMM: their common input can be cast to e4m3 once, by its
+    producer."""
+    return all(fp8.is_blockwise(m) for m in lins)
+
+
+def _ln_fp8(lins, x, **kw):
+    """The LayerNorm feeding ``lins`` with its e4m3 cast fused in when they all take the same FP8 input: per 128-channel
+    group (PerBlock) or per row (PerRow); None when they do not."""
+    if _blockwise(*lins):
+        return ops.ln_modulate_fp8_blocks(x, **kw)
+    if _rowwise(*lins):
+        return ops.ln_modulate_fp8(x, **kw)
+    return None
 
 
 def rope_angles(max_seq_len: int, dim: int, theta: float = 10000.0) -> torch.Tensor:
@@ -409,7 +428,9 @@ class CausalWanModel(nn.Module):
         if cache is not None and cache["is_init"]:
             k, v = cache["k"], cache["v"]
         else:
-            if _rowwise(ca.k, ca.v):
+            if _blockwise(ca.k, ca.v):
+                ctx = ops.fp8_quantize_blocks(ctx)      # one per-group cast of the prompt feeds both projections
+            elif _rowwise(ca.k, ca.v):
                 ctx = ops.fp8_quantize_rows(ctx)        # one per-row cast of the prompt feeds both projections
             k = _linear(ctx, ca.k)
             ops.rmsnorm(k, ca.norm_k.weight, ca.eps, out=k)
@@ -472,31 +493,30 @@ class CausalWanModel(nn.Module):
         r0 = 0 if self.sp is None else self.sp.rank * x.shape[0]       # global index of my first row
         emod = ops.add_modulation(blk.modulation, e0)                    # [F, 6, D]
         sa, ca = blk.self_attn, blk.cross_attn
-        # PerRow FP8: a LayerNorm whose every consumer is a row-scaled FP8 linear writes e4m3 bytes + row scales
-        # instead of its bf16 output (ln_modulate_fp8); `buf` is the bf16 scratch row buffer while there is one
-        if _rowwise(*((sa.to_qkv,) if sa.fused_projections else (sa.q, sa.k, sa.v))):
-            h = ops.ln_modulate_fp8(x, eps=blk.eps, mod=emod, shift_idx=0, scale_idx=1, rows_per_frame=fs,
-                                    row_offset=r0)
-            buf = None
-        else:
+        # PerRow / PerBlock FP8: a LayerNorm whose every consumer is a row- (block-) scaled FP8 linear writes e4m3
+        # bytes + row (group) scales instead of its bf16 output (ln_modulate_fp8[_blocks]); `buf` is the bf16 scratch
+        # row buffer while there is one
+        h = _ln_fp8((sa.to_qkv,) if sa.fused_projections else (sa.q, sa.k, sa.v), x, eps=blk.eps, mod=emod,
+                    shift_idx=0, scale_idx=1, rows_per_frame=fs, row_offset=r0)
+        buf = None
+        if h is None:
             h = buf = ops.ln_modulate(x, eps=blk.eps, mod=emod, shift_idx=0, scale_idx=1, rows_per_frame=fs,
                                       row_offset=r0)
         y = self._self_attention(blk, h, grid, kv_cache, current_start, mask)
         _linear(y, sa.o, epilogue=ops.EPI_BIAS_GATE_RES, residual=x,
                  gate=emod[:, 2], rows_per_gate=fs, out=x, row_offset=r0)
         n3 = blk.norm3
-        if isinstance(n3, nn.LayerNorm) and _rowwise(ca.q):
-            hc = ops.ln_modulate_fp8(x, eps=n3.eps, weight=n3.weight, bias=n3.bias)
-        elif isinstance(n3, nn.LayerNorm):
-            hc = buf = ops.ln_modulate(x, eps=n3.eps, weight=n3.weight, bias=n3.bias, out=buf)
+        if isinstance(n3, nn.LayerNorm):
+            hc = _ln_fp8((ca.q,), x, eps=n3.eps, weight=n3.weight, bias=n3.bias)
+            if hc is None:
+                hc = buf = ops.ln_modulate(x, eps=n3.eps, weight=n3.weight, bias=n3.bias, out=buf)
         else:
             hc = x          # cross_attn_norm=False: the residual stream itself; `buf` stays the scratch buffer
         y = self._cross_attention(blk, hc, ctx, crossattn_cache)
         _linear(y, ca.o, epilogue=ops.EPI_BIAS_RES, residual=x, out=x)
-        if _rowwise(blk.ffn[0]):
-            h = ops.ln_modulate_fp8(x, eps=blk.eps, mod=emod, shift_idx=3, scale_idx=4, rows_per_frame=fs,
-                                    row_offset=r0)
-        else:
+        h = _ln_fp8((blk.ffn[0],), x, eps=blk.eps, mod=emod, shift_idx=3, scale_idx=4, rows_per_frame=fs,
+                    row_offset=r0)
+        if h is None:
             h = ops.ln_modulate(x, eps=blk.eps, mod=emod, shift_idx=3, scale_idx=4, rows_per_frame=fs, out=buf,
                                 row_offset=r0)
         hid = _linear(h, blk.ffn[0], epilogue=ops.EPI_BIAS_GELU)

@@ -14,7 +14,8 @@ resolving to the reference checkout, independent of the ``sys.path`` order:
     wan.modules.causal_model   -> realtime_video_b200.dit           (CausalWanModel; wan/modules/causal_model.py:526)
     torchao.quantization.quant_api -> realtime_video_b200.fp8       (quantize_, Float8DynamicActivationFloat8WeightConfig,
                                                                      PerTensor: the `enable_fp8` lines release_server.py:179-182;
-                                                                     PerRow: the same lines with granularity=PerRow() also resolve)
+                                                                     PerRow: the same lines with granularity=PerRow() also resolve;
+                                                                     PerBlock: granularity=[PerBlock([1, 128]), PerBlock([128, 128])])
     torchao.float8.inference   -> realtime_video_b200.fp8           (Float8MMConfig, where torchao defines it: the same lines
                                                                      with mm_config=Float8MMConfig(use_fast_accum=True))
 
@@ -42,7 +43,7 @@ ALIASES = {
     "demo_utils.vae": "realtime_video_b200.vae",
     "wan.modules.causal_model": "realtime_video_b200.dit",
     # `enable_fp8: true` (release_server.py:179-182): quantize_ / Float8DynamicActivationFloat8WeightConfig / PerTensor
-    # (or PerRow)
+    # (or PerRow, or PerBlock)
     "torchao.quantization.quant_api": "realtime_video_b200.fp8",
     # Float8MMConfig, the mm_config argument of the config above, under the module torchao defines it in
     "torchao.float8.inference": "realtime_video_b200.fp8",

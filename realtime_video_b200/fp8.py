@@ -26,6 +26,14 @@ accumulator keeps fewer mantissa bits than fp32 and the promoted kernel is the o
 with.  ``KR_FP8_FAST_ACCUM=1`` in the environment makes ``quantize_`` calls that pass no ``mm_config`` choose fast
 accumulation, so the reference's unmodified lines reach it.  Weights and scales are the same bytes in both modes.
 
+``granularity=[PerBlock([1, 128]), PerBlock([128, 128])]`` is block scaling (the DeepSeek-V3 FP8 recipe; torchao's
+``PerBlock``): one scale per 1 x 128 group of an activation row and one per 128 x 128 block of the weight, so a
+channel that is large in every token sets the scale of its own 128-channel group instead of every row's.  The block
+schedule then runs ``kr_gemm_fp8_blockwise`` (each 128-wide k-block's partial is multiplied by its two scales when it is
+promoted to fp32) fed by ``kr_ln_modulate_fp8_blocks`` or ``kr_fp8_quantize_blocks``.  Block scales need a partial sum
+per k-block, so this granularity exists only with promoted accumulation: ``Float8MMConfig(use_fast_accum=True)`` with
+``PerBlock`` raises ``NotImplementedError``, and ``KR_FP8_FAST_ACCUM=1`` does not apply to it.
+
 Numerics are a separate tier from the bf16 headline: e4m3 has 3 mantissa bits; tests state the tolerance against the
 fp8 oracle (same quantisation, fp32 matmul) and against the bf16 path.
 """
@@ -48,6 +56,26 @@ class PerRow:
     """Granularity marker (torchao.quantization.PerRow): per-row activation scales, per-output-channel weight scales."""
 
 
+BLOCK = 128
+
+
+class PerBlock:
+    """Granularity marker (torchao.quantization.PerBlock): one scale per ``block_size`` block.  Accepted only as the
+    pair ``[PerBlock([1, 128]), PerBlock([128, 128])]`` (1 x 128 activation groups, 128 x 128 weight blocks)."""
+
+    def __init__(self, block_size):
+        self.block_size = tuple(int(b) for b in block_size)
+
+    def __eq__(self, other):
+        return isinstance(other, PerBlock) and other.block_size == self.block_size
+
+    def __hash__(self):
+        return hash(("PerBlock", self.block_size))
+
+    def __repr__(self):
+        return f"PerBlock({list(self.block_size)})"
+
+
 @dataclass(frozen=True)
 class Float8MMConfig:
     """torchao.float8.inference.Float8MMConfig, field for field.  ``use_fast_accum=True`` runs the FP8 GEMM that
@@ -68,15 +96,24 @@ def _fast_accum_default() -> bool:
 
 
 class Float8DynamicActivationFloat8WeightConfig:
-    """``granularity``: ``PerTensor()`` or ``PerRow()``, alone or as an (activation, weight) pair of the same kind.
-    ``mm_config``: a :class:`Float8MMConfig`, or None for promoted accumulation (torchao's None means
-    ``use_fast_accum=True``; see the module docstring) unless ``KR_FP8_FAST_ACCUM=1``."""
+    """``granularity``: ``PerTensor()`` or ``PerRow()``, alone or as an (activation, weight) pair of the same kind, or
+    exactly the pair ``[PerBlock([1, 128]), PerBlock([128, 128])]``.  ``mm_config``: a :class:`Float8MMConfig`, or None
+    for promoted accumulation (torchao's None means ``use_fast_accum=True``; see the module docstring) unless
+    ``KR_FP8_FAST_ACCUM=1``.  ``PerBlock`` is promoted only: ``use_fast_accum=True`` with it raises."""
 
     def __init__(self, granularity=None, mm_config=None, **unused):
         if mm_config is not None and not isinstance(mm_config, Float8MMConfig):
             raise TypeError(f"mm_config must be a Float8MMConfig or None, got {type(mm_config).__name__}")
         self.mm_config = mm_config
         g = PerTensor() if granularity is None else granularity
+        if isinstance(g, PerBlock) or (isinstance(g, (list, tuple)) and any(isinstance(x, PerBlock) for x in g)):
+            self.granularity = self._per_block(g)
+            if mm_config is not None and mm_config.use_fast_accum:
+                raise NotImplementedError(
+                    "PerBlock with Float8MMConfig(use_fast_accum=True) is not implemented: block scales are applied "
+                    "to each 128-wide k-block's partial sum when it is promoted to fp32, and fast accumulation keeps "
+                    "no such partial")
+            return
         if isinstance(g, (list, tuple)):
             if len(g) != 2:
                 raise ValueError(f"granularity pair must have two entries, got {len(g)}")
@@ -87,6 +124,19 @@ class Float8DynamicActivationFloat8WeightConfig:
         if not isinstance(g, (PerTensor, PerRow)):
             raise NotImplementedError(f"granularity {type(g).__name__} is not implemented (PerTensor or PerRow)")
         self.granularity = g
+
+    @staticmethod
+    def _per_block(g):
+        if not isinstance(g, (list, tuple)) or len(g) != 2:
+            raise ValueError("PerBlock granularity is an (activation, weight) pair: "
+                             "[PerBlock([1, 128]), PerBlock([128, 128])]")
+        if not all(isinstance(x, PerBlock) for x in g):
+            raise ValueError("activation and weight granularity must be of the same kind, got "
+                             f"{type(g[0]).__name__} and {type(g[1]).__name__}")
+        if g[0].block_size != (1, BLOCK) or g[1].block_size != (BLOCK, BLOCK):
+            raise NotImplementedError(f"PerBlock block sizes {list(g[0].block_size)} / {list(g[1].block_size)} are "
+                                      f"not implemented (activation [1, {BLOCK}], weight [{BLOCK}, {BLOCK}])")
+        return g[0]
 
 
 @torch.no_grad()
@@ -107,9 +157,29 @@ def quantize_weight_rows(w: torch.Tensor):
     return q.view(torch.uint8).contiguous(), (amax / E4M3_MAX).squeeze(1).contiguous()
 
 
+@torch.no_grad()
+def quantize_weight_blocks(w: torch.Tensor):
+    """w [N, K] (N, K multiples of 128) -> (e4m3 bytes as uint8 [N, K], fp32 [N/128, K/128] dequantisation scales
+    amax_b / 448), one per 128 x 128 block: w_q[b] = sat(w[b] * 448 / amax_b), a true division as in
+    :func:`quantize_weight_rows`; an all-zero block gets amax 1e-12."""
+    N, K = w.shape
+    if N % BLOCK or K % BLOCK:
+        raise ValueError(f"quantize_weight_blocks: [{N}, {K}] is not a whole number of {BLOCK} x {BLOCK} blocks")
+    wb = w.detach().float().reshape(N // BLOCK, BLOCK, K // BLOCK, BLOCK)
+    amax = wb.abs().amax(dim=(1, 3), keepdim=True).clamp(min=1e-12)
+    mul = torch.full_like(amax, E4M3_MAX) / amax
+    q = (wb * mul).clamp(-E4M3_MAX, E4M3_MAX).to(torch.float8_e4m3fn).reshape(N, K)
+    return q.view(torch.uint8).contiguous(), (amax / E4M3_MAX).reshape(N // BLOCK, K // BLOCK).contiguous()
+
+
 def is_rowwise(lin: nn.Module) -> bool:
     """True when :func:`quantize_` attached per-row (PerRow) FP8 weights to ``lin``."""
     return isinstance(getattr(lin, "_kr_fp8_granularity", None), PerRow)
+
+
+def is_blockwise(lin: nn.Module) -> bool:
+    """True when :func:`quantize_` attached block-scaled (PerBlock) FP8 weights to ``lin``."""
+    return isinstance(getattr(lin, "_kr_fp8_granularity", None), PerBlock)
 
 
 def is_fast_accum(lin: nn.Module) -> bool:
@@ -122,14 +192,17 @@ def quantize_(module: nn.Module, config=None, filter_fn=None) -> nn.Module:
     """In-place, like torchao's: every ``nn.Linear`` inside the DiT blocks of ``module`` (a WanDiffusionWrapper, a
     CausalWanModel or any container of CausalWanAttentionBlock) gets FP8 weights.  The bf16 weights stay in place
     (state_dict unchanged); call ``dequantize_`` to go back.  PerTensor attaches ``(w_q, scale_w float)``, PerRow
-    ``(w_q, scale_w fp32 [N])`` on the weight's device.  The accumulation mode of ``config.mm_config`` is recorded
+    ``(w_q, scale_w fp32 [N])``, PerBlock ``(w_q, scale_w fp32 [N/128, K/128])`` (only to Linears with K % 128 == 0)
+    on the weight's device.  The accumulation mode of ``config.mm_config`` is recorded
     beside them; the weights and scales do not depend on it."""
     if config is not None and not isinstance(config, Float8DynamicActivationFloat8WeightConfig):
         raise NotImplementedError(f"unsupported quantisation config {type(config).__name__}")
     gran = config.granularity if config is not None else PerTensor()
-    quant = quantize_weight_rows if isinstance(gran, PerRow) else quantize_weight
+    blocks = isinstance(gran, PerBlock)
+    quant = quantize_weight_blocks if blocks else quantize_weight_rows if isinstance(gran, PerRow) else quantize_weight
     mm = config.mm_config if config is not None else None
-    fast = _fast_accum_default() if mm is None else mm.use_fast_accum
+    # PerBlock is promoted only (the config rejects use_fast_accum=True); the environment switch does not apply to it
+    fast = False if blocks else _fast_accum_default() if mm is None else mm.use_fast_accum
     from .dit import CausalWanAttentionBlock
     n = 0
     for blk in module.modules():
@@ -137,7 +210,7 @@ def quantize_(module: nn.Module, config=None, filter_fn=None) -> nn.Module:
             continue
         for name, lin in blk.named_modules():
             if isinstance(lin, nn.Linear) and lin.weight.shape[0] % 256 == 0 and lin.weight.shape[1] % 16 == 0 and \
-                    (filter_fn is None or filter_fn(lin, name)):
+                    (not blocks or lin.weight.shape[1] % BLOCK == 0) and (filter_fn is None or filter_fn(lin, name)):
                 lin._kr_fp8 = quant(lin.weight)
                 lin._kr_fp8_granularity = gran
                 if fast:
