@@ -14,6 +14,18 @@
     }                                         \
   } while (0)
 
+// The GEMM arguments every kr_gemm* entry point shares after its operands and scales.
+static kr::GemmParams gemm_params(const void* bias, void* out, int ldc, int M, int N, int K, const void* residual,
+                                  int ldr, const void* gate, int gate_stride, int rows_per_gate, void* out2, int ldc2,
+                                  int n_split, int row_offset, float alpha = 1.0f) {
+  kr::GemmParams p;
+  p.out = out; p.bias = bias; p.residual = residual; p.gate = gate;
+  p.M = M; p.N = N; p.K = K; p.ldc = ldc; p.ldr = ldr; p.gate_stride = gate_stride;
+  p.rows_per_gate = rows_per_gate; p.alpha = alpha;
+  p.out2 = out2; p.ldc2 = ldc2; p.n_split = n_split; p.row_offset = row_offset;
+  return p;
+}
+
 extern "C" {
 
 int kr_version(void) { return 100; }
@@ -40,11 +52,8 @@ int kr_gemm_ws(int dtype, int epilogue, const void* a, int lda, const void* w, i
                void* stream) {
   KR_REQUIRE(a && w && out, "null a/w/out");
   KR_REQUIRE(dtype == 0 || dtype == 1, "dtype must be 0 (bf16) or 1 (fp16)");
-  kr::GemmParams p;
-  p.out = out; p.bias = bias; p.residual = residual; p.gate = gate;
-  p.M = M; p.N = N; p.K = K; p.ldc = ldc; p.ldr = ldr; p.gate_stride = gate_stride;
-  p.rows_per_gate = rows_per_gate; p.alpha = alpha;
-  p.out2 = out2; p.ldc2 = ldc2; p.n_split = n_split; p.row_offset = row_offset;
+  const kr::GemmParams p = gemm_params(bias, out, ldc, M, N, K, residual, ldr, gate, gate_stride, rows_per_gate, out2,
+                                       ldc2, n_split, row_offset, alpha);
   return kr::gemm_tn(dtype, epilogue, a, lda, w, ldw, p, static_cast<cudaStream_t>(stream), workspace, workspace_bytes);
 }
 
@@ -58,11 +67,8 @@ int kr_gemm_fp8(int epilogue, const void* a, int lda, const void* w, int ldw, co
                 const void* gate, int gate_stride, int rows_per_gate, void* out2, int ldc2, int n_split, int row_offset,
                 void* stream) {
   KR_REQUIRE(a && w && out, "null a/w/out");
-  kr::GemmParams p;
-  p.out = out; p.bias = bias; p.residual = residual; p.gate = gate;
-  p.M = M; p.N = N; p.K = K; p.ldc = ldc; p.ldr = ldr; p.gate_stride = gate_stride;
-  p.rows_per_gate = rows_per_gate; p.alpha = 1.0f;
-  p.out2 = out2; p.ldc2 = ldc2; p.n_split = n_split; p.row_offset = row_offset;
+  const kr::GemmParams p = gemm_params(bias, out, ldc, M, N, K, residual, ldr, gate, gate_stride, rows_per_gate, out2,
+                                       ldc2, n_split, row_offset);
   return kr::gemm_fp8_tn(epilogue, a, lda, w, ldw, p, scale_a, scale_w, static_cast<cudaStream_t>(stream));
 }
 
@@ -98,11 +104,8 @@ int kr_gemm_fp8_rowwise(int epilogue, const void* a, int lda, const void* w, int
   KR_REQUIRE(a && w && out, "null a/w/out");
   KR_REQUIRE(scale_a && scale_w, "null scale_a/scale_w");
   KR_REQUIRE_LINKED(gemm_fp8_rowwise_tn);
-  kr::GemmParams p;
-  p.out = out; p.bias = bias; p.residual = residual; p.gate = gate;
-  p.M = M; p.N = N; p.K = K; p.ldc = ldc; p.ldr = ldr; p.gate_stride = gate_stride;
-  p.rows_per_gate = rows_per_gate; p.alpha = 1.0f;
-  p.out2 = out2; p.ldc2 = ldc2; p.n_split = n_split; p.row_offset = row_offset;
+  const kr::GemmParams p = gemm_params(bias, out, ldc, M, N, K, residual, ldr, gate, gate_stride, rows_per_gate, out2,
+                                       ldc2, n_split, row_offset);
   return kr::gemm_fp8_rowwise_tn(epilogue, a, lda, w, ldw, p, scale_a, scale_w, static_cast<cudaStream_t>(stream));
 }
 
@@ -123,11 +126,8 @@ int kr_gemm_fp8_fast(int epilogue, const void* a, int lda, const void* w, int ld
   KR_REQUIRE(scale_a, "null scale_a");
   KR_REQUIRE_FP8_FAST_SHAPE();
   KR_REQUIRE_LINKED(gemm_fp8_fast_tn);
-  kr::GemmParams p;
-  p.out = out; p.bias = bias; p.residual = residual; p.gate = gate;
-  p.M = M; p.N = N; p.K = K; p.ldc = ldc; p.ldr = ldr; p.gate_stride = gate_stride;
-  p.rows_per_gate = rows_per_gate; p.alpha = 1.0f;
-  p.out2 = out2; p.ldc2 = ldc2; p.n_split = n_split; p.row_offset = row_offset;
+  const kr::GemmParams p = gemm_params(bias, out, ldc, M, N, K, residual, ldr, gate, gate_stride, rows_per_gate, out2,
+                                       ldc2, n_split, row_offset);
   return kr::gemm_fp8_fast_tn(epilogue, a, lda, w, ldw, p, scale_a, scale_w, static_cast<cudaStream_t>(stream));
 }
 
@@ -139,11 +139,8 @@ int kr_gemm_fp8_rowwise_fast(int epilogue, const void* a, int lda, const void* w
   KR_REQUIRE(scale_a && scale_w, "null scale_a/scale_w");
   KR_REQUIRE_FP8_FAST_SHAPE();
   KR_REQUIRE_LINKED(gemm_fp8_rowwise_fast_tn);
-  kr::GemmParams p;
-  p.out = out; p.bias = bias; p.residual = residual; p.gate = gate;
-  p.M = M; p.N = N; p.K = K; p.ldc = ldc; p.ldr = ldr; p.gate_stride = gate_stride;
-  p.rows_per_gate = rows_per_gate; p.alpha = 1.0f;
-  p.out2 = out2; p.ldc2 = ldc2; p.n_split = n_split; p.row_offset = row_offset;
+  const kr::GemmParams p = gemm_params(bias, out, ldc, M, N, K, residual, ldr, gate, gate_stride, rows_per_gate, out2,
+                                       ldc2, n_split, row_offset);
   return kr::gemm_fp8_rowwise_fast_tn(epilogue, a, lda, w, ldw, p, scale_a, scale_w,
                                       static_cast<cudaStream_t>(stream));
 }
@@ -180,11 +177,8 @@ int kr_gemm_fp8_blockwise(int epilogue, const void* a, int lda, const void* w, i
   KR_REQUIRE(lda % 16 == 0 && ldw % 16 == 0 && lda >= K && ldw >= K && ldc % 8 == 0 && ldc > 0 && ld_sa >= M,
              "pitches: lda / ldw >= K and % 16 == 0, ldc % 8 == 0, ld_sa >= M");
   KR_REQUIRE_LINKED(gemm_fp8_blockwise_tn);
-  kr::GemmParams p;
-  p.out = out; p.bias = bias; p.residual = residual; p.gate = gate;
-  p.M = M; p.N = N; p.K = K; p.ldc = ldc; p.ldr = ldr; p.gate_stride = gate_stride;
-  p.rows_per_gate = rows_per_gate; p.alpha = 1.0f;
-  p.out2 = out2; p.ldc2 = ldc2; p.n_split = n_split; p.row_offset = row_offset;
+  const kr::GemmParams p = gemm_params(bias, out, ldc, M, N, K, residual, ldr, gate, gate_stride, rows_per_gate, out2,
+                                       ldc2, n_split, row_offset);
   return kr::gemm_fp8_blockwise_tn(epilogue, a, lda, w, ldw, p, scale_a, ld_sa, scale_w,
                                    static_cast<cudaStream_t>(stream));
 }

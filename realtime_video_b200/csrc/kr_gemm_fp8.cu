@@ -11,20 +11,21 @@
 // followed by torch._scaled_mm (cuBLASLt FP8, fp32 accumulation, bf16 output) — here a hand-written
 // wgmma e4m3 kernel with the same fused epilogues as the bf16 GEMM (bias, GELU, gate + residual, ...).
 // torchao is absent from the image: the algorithm is restated from its published definition (oracle/fp8_oracle.py).
-// granularity=PerRow() gives one scale per activation row and one per weight output channel: the same kernel, with
-// the two scale vectors applied in the epilogue (torch._scaled_mm with scale_a [M, 1], scale_b [1, N]);
-// oracle/fp8_rowwise_oracle.py restates it.
+// granularity=PerRow() gives one scale per activation row and one per weight output channel, applied in the epilogue
+// (torch._scaled_mm with scale_a [M, 1], scale_b [1, N]); oracle/fp8_rowwise_oracle.py restates it.
+// granularity=PerBlock() ([1, 128] activations / [128, 128] weights, the DeepSeek-V3 recipe) multiplies each k-block's
+// partial by sa[kb][row] * sw[n_blk][kb] at the promotion; oracle/fp8_blockwise_oracle.py restates it.
 //
-// Kernel structure = kr_gemm.cu (persistent 1 CTA/SM, two consumer warpgroups with register accumulators, a TMA
-// warpgroup), with byte-sized elements: a 128-byte swizzle row holds 128 k-elements, one wgmma consumes K = 32
-// (32 bytes).  Two kernels of that structure differ in how they accumulate:
-//   gemm_fp8_kernel      (promoted, the default): each 128-wide k-block is accumulated separately and added to the
-//                        fp32 registers (the e4m3 wgmma adder keeps fewer mantissa bits), so the tile is 128 x 128
-//                        to leave registers for the partial;
-//   gemm_fp8_fast_kernel (torchao Float8MMConfig(use_fast_accum=True) = torch._scaled_mm(use_fast_accum=True)): the
-//                        wgmma accumulates in place across the whole K with one group in flight, like the 16-bit
-//                        GEMM, so the registers hold a 128 x 256 tile (m64n256k32, half the shared-memory operand
-//                        bytes per FLOP) and the tensor cores are not drained after every k-block.
+// One kernel template, gemm_fp8_kernel<kEpi, kScale, kFast>, with the structure of kr_gemm.cu (persistent 1 CTA/SM,
+// two consumer warpgroups with register accumulators, a TMA warpgroup) and byte-sized elements: a 128-byte swizzle row
+// holds 128 k-elements, one wgmma consumes K = 32 (32 bytes).  kFast selects how it accumulates:
+//   promoted (default): each 128-wide k-block is accumulated separately and added to the fp32 registers (the e4m3
+//            wgmma adder keeps fewer mantissa bits), on a 128 x 128 tile to leave registers for the partial.  Block
+//            scales are applied at this promotion; the tile then spans one weight block in N and one activation
+//            group per k-block, so the epilogue applies no scale;
+//   fast     (torch._scaled_mm(use_fast_accum=True)): the wgmma accumulates in place across the whole K with one group
+//            in flight, like the 16-bit GEMM, on a 128 x 256 tile (m64n256k32, half the shared-memory operand bytes
+//            per FLOP) without draining the tensor cores after every k-block.
 #include "kr_common.cuh"
 #include "kr_gemm_epi.cuh"
 #include "kr_ops.h"
@@ -34,33 +35,45 @@
 namespace kr {
 
 namespace {
-constexpr int F8_BM = 128, F8_BN = 128, F8_BK = 128 /* elements = bytes */;
+constexpr int F8_BM = 128, F8_BK = 128 /* elements = bytes */;
 constexpr int F8_THREADS = 384, F8_STAGES = 4;
-constexpr int F8_A_BYTES = F8_BM * F8_BK, F8_B_BYTES = F8_BN * F8_BK, F8_STAGE_BYTES = F8_A_BYTES + F8_B_BYTES;
+constexpr int F8_A_BYTES = F8_BM * F8_BK;
 constexpr int F8_SCR_BYTES = 8 * kEpiScrFloats * 4;
-constexpr int F8_SMEM = F8_STAGES * F8_STAGE_BYTES + F8_SCR_BYTES + 1024 + 256;
+__host__ __device__ constexpr int f8_bn(bool fast) { return fast ? 256 : 128; }
+constexpr int f8_smem(bool fast) { return F8_STAGES * (F8_A_BYTES + f8_bn(fast) * F8_BK) + F8_SCR_BYTES + 1024 + 256; }
+static_assert(f8_smem(true) <= 227 * 1024, "4 stages of 16 KB A + 32 KB W and the epilogue scratch fit one SM");
+
+enum Fp8Scale { F8_SCALE_TENSOR, F8_SCALE_ROW, F8_SCALE_BLOCK };
+
+// The I-th scale argument: a mode's scale arguments are separate kernel parameters, as many as the mode needs.
+template <int I, typename T, typename... R>
+__host__ __device__ __forceinline__ auto f8_arg(T t, R... r) {
+  if constexpr (I == 0) return t;
+  else return f8_arg<I - 1>(r...);
+}
 }  // namespace
 
-// per tensor: scale_a -> one fp32 in device memory, scale_w a float; per row: scale_a -> [M], scale_w -> [N] fp32
-template <bool kRowwise> struct Fp8ScaleW { using type = float; };
-template <> struct Fp8ScaleW<true> { using type = const float*; };
-
-template <int kEpi, bool kRowwise>
+// The scale arguments by kScale.  tensor: scale_a -> one fp32, float scale_w.  row: scale_a -> [M], scale_w -> [N].
+// block: scale_a -> fp32 [K/128, ld_sa] (k-block-major: one k-block's row scales are contiguous), then long ld_sa and
+// scale_w -> fp32 [N/128, K/128].
+template <int kEpi, int kScale, bool kFast, typename... ScaleW>
 __global__ void __launch_bounds__(F8_THREADS, 1)
 gemm_fp8_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
-                const GemmParams p, const float* __restrict__ scale_a, const typename Fp8ScaleW<kRowwise>::type scale_w) {
+                const GemmParams p, const float* __restrict__ scale_a, ScaleW... scale_w) {
+  static_assert(!(kFast && kScale == F8_SCALE_BLOCK), "block scales are applied at the promotion");
+  constexpr int BN = f8_bn(kFast), B_BYTES = BN * F8_BK, STAGE_BYTES = F8_A_BYTES + B_BYTES;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
                                              ~static_cast<uintptr_t>(1023));
   uint8_t* smem_a = smem;
   uint8_t* smem_b = smem + F8_STAGES * F8_A_BYTES;
-  float* scratch = reinterpret_cast<float*>(smem + F8_STAGES * F8_STAGE_BYTES);
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + F8_STAGES * F8_STAGE_BYTES + F8_SCR_BYTES);
+  float* scratch = reinterpret_cast<float*>(smem + F8_STAGES * STAGE_BYTES);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + F8_STAGES * STAGE_BYTES + F8_SCR_BYTES);
   uint64_t* full_bar = bars;
   uint64_t* empty_bar = bars + F8_STAGES;
 
   const int warp = threadIdx.x >> 5;
-  const int num_m = (p.M + F8_BM - 1) / F8_BM, num_n = p.N / F8_BN, num_tiles = num_m * num_n;
+  const int num_m = (p.M + F8_BM - 1) / F8_BM, num_n = p.N / BN, num_tiles = num_m * num_n;
   const int num_k = (p.K + F8_BK - 1) / F8_BK;
 
   if (threadIdx.x == 256) {
@@ -83,9 +96,9 @@ gemm_fp8_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constan
         const int m_blk = tile % num_m, n_blk = tile / num_m;
         for (int kb = 0; kb < num_k; ++kb) {
           mbar_wait(&empty_bar[stage], phase ^ 1);
-          mbar_expect_tx(&full_bar[stage], F8_STAGE_BYTES);
+          mbar_expect_tx(&full_bar[stage], STAGE_BYTES);
           tma_load_2d(smem_a + stage * F8_A_BYTES, &tmap_a, &full_bar[stage], kb * F8_BK, m_blk * F8_BM);
-          tma_load_2d(smem_b + stage * F8_B_BYTES, &tmap_b, &full_bar[stage], kb * F8_BK, n_blk * F8_BN);
+          tma_load_2d(smem_b + stage * B_BYTES, &tmap_b, &full_bar[stage], kb * F8_BK, n_blk * BN);
           if (++stage == F8_STAGES) {
             stage = 0;
             phase ^= 1;
@@ -100,181 +113,33 @@ gemm_fp8_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constan
   const uint32_t a_base = smem_u32(smem_a) + wg * 64 * F8_BK, b_base = smem_u32(smem_b);
   float* scr = scratch + warp * kEpiScrFloats;
   float s = 1.f;
-  if constexpr (!kRowwise) s = __ldg(scale_a) * scale_w;   // dequantisation: per-tensor activation x weight scale
+  if constexpr (kScale == F8_SCALE_TENSOR) s = __ldg(scale_a) * f8_arg<0>(scale_w...);   // per-tensor dequantisation
   int stage = 0;
   uint32_t phase = 0;
   for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
     const int m_blk = tile % num_m, n_blk = tile / num_m;
-    float acc[F8_BN / 2];
-    gemm_mainloop<F8_BN, 2>(acc, a_base, b_base, F8_A_BYTES, F8_B_BYTES, F8_STAGES, full_bar, empty_bar, stage, phase,
-                            0, num_k);
-    if constexpr (kRowwise)
-      gemm_frag_epilogue<F8_BN, true, kEpi, true>(acc, scr, m_blk * F8_BM + wg * 64 + (warp & 3) * 16, n_blk * F8_BN,
-                                                  F8_BN, s, p, scale_a, scale_w);
-    else
-      gemm_frag_epilogue<F8_BN, true, kEpi>(acc, scr, m_blk * F8_BM + wg * 64 + (warp & 3) * 16, n_blk * F8_BN, F8_BN,
-                                            s, p);
-  }
-}
-
-// Fast accumulation: the body of gemm_fp8_kernel on a 128 x 256 tile, with gemm_mainloop accumulating in place (one
-// wgmma group in flight, a stage released when the group that read it has retired).  A kernel of its own rather than
-// a shared body: the promoted kernel must keep its machine code bit for bit, and routing it through a common
-// function changed its register allocation.
-namespace {
-constexpr int F8F_BN = 256, F8F_B_BYTES = F8F_BN * F8_BK, F8F_STAGE_BYTES = F8_A_BYTES + F8F_B_BYTES;
-constexpr int F8F_SMEM = F8_STAGES * F8F_STAGE_BYTES + F8_SCR_BYTES + 1024 + 256;
-static_assert(F8F_SMEM <= 227 * 1024, "4 stages of 16 KB A + 32 KB W and the epilogue scratch fit one SM");
-}  // namespace
-
-template <int kEpi, bool kRowwise>
-__global__ void __launch_bounds__(F8_THREADS, 1)
-gemm_fp8_fast_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
-                     const GemmParams p, const float* __restrict__ scale_a,
-                     const typename Fp8ScaleW<kRowwise>::type scale_w) {
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
-                                             ~static_cast<uintptr_t>(1023));
-  uint8_t* smem_a = smem;
-  uint8_t* smem_b = smem + F8_STAGES * F8_A_BYTES;
-  float* scratch = reinterpret_cast<float*>(smem + F8_STAGES * F8F_STAGE_BYTES);
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + F8_STAGES * F8F_STAGE_BYTES + F8_SCR_BYTES);
-  uint64_t* full_bar = bars;
-  uint64_t* empty_bar = bars + F8_STAGES;
-
-  const int warp = threadIdx.x >> 5;
-  const int num_m = (p.M + F8_BM - 1) / F8_BM, num_n = p.N / F8F_BN, num_tiles = num_m * num_n;
-  const int num_k = (p.K + F8_BK - 1) / F8_BK;
-
-  if (threadIdx.x == 256) {
-    prefetch_tmap(&tmap_a);
-    prefetch_tmap(&tmap_b);
-    for (int i = 0; i < F8_STAGES; ++i) {
-      mbar_init(&full_bar[i], 1);
-      mbar_init(&empty_bar[i], 2);
+    if constexpr (kScale == F8_SCALE_BLOCK) {
+      const int row0 = m_blk * F8_BM + wg * 64 + (warp & 3) * 16;
+      const int r = row0 + ((threadIdx.x & 31) >> 2);
+      BlockScales bs;
+      bs.sa0 = r < p.M ? scale_a + r : nullptr;
+      bs.sa1 = r + 8 < p.M ? scale_a + r + 8 : nullptr;
+      bs.ld = f8_arg<0>(scale_w...);
+      bs.sw = f8_arg<1>(scale_w...) + static_cast<long>(n_blk) * num_k;
+      float acc[BN / 2];
+      gemm_mainloop<BN, 2, 1, true, true>(acc, a_base, b_base, F8_A_BYTES, B_BYTES, F8_STAGES, full_bar, empty_bar,
+                                          stage, phase, 0, num_k, bs);
+      gemm_frag_epilogue<BN, true, kEpi>(acc, scr, row0, n_blk * BN, BN, 1.f, p);
+    } else {
+      float acc[BN / 2];
+      gemm_mainloop<BN, 2, 1, !kFast>(acc, a_base, b_base, F8_A_BYTES, B_BYTES, F8_STAGES, full_bar, empty_bar, stage,
+                                      phase, 0, num_k);
+      if constexpr (kScale == F8_SCALE_ROW)
+        gemm_frag_epilogue<BN, true, kEpi, true>(acc, scr, m_blk * F8_BM + wg * 64 + (warp & 3) * 16, n_blk * BN, BN,
+                                                 s, p, scale_a, f8_arg<0>(scale_w...));
+      else
+        gemm_frag_epilogue<BN, true, kEpi>(acc, scr, m_blk * F8_BM + wg * 64 + (warp & 3) * 16, n_blk * BN, BN, s, p);
     }
-    fence_barrier_init();
-  }
-  __syncthreads();
-
-  if (warp >= 8) {
-    producer_regs();
-    if (warp == 8 && elect_one()) {
-      int stage = 0;
-      uint32_t phase = 0;
-      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-        const int m_blk = tile % num_m, n_blk = tile / num_m;
-        for (int kb = 0; kb < num_k; ++kb) {
-          mbar_wait(&empty_bar[stage], phase ^ 1);
-          mbar_expect_tx(&full_bar[stage], F8F_STAGE_BYTES);
-          tma_load_2d(smem_a + stage * F8_A_BYTES, &tmap_a, &full_bar[stage], kb * F8_BK, m_blk * F8_BM);
-          tma_load_2d(smem_b + stage * F8F_B_BYTES, &tmap_b, &full_bar[stage], kb * F8_BK, n_blk * F8F_BN);
-          if (++stage == F8_STAGES) {
-            stage = 0;
-            phase ^= 1;
-          }
-        }
-      }
-    }
-    return;
-  }
-  consumer_regs();
-  const int wg = warp >> 2;
-  const uint32_t a_base = smem_u32(smem_a) + wg * 64 * F8_BK, b_base = smem_u32(smem_b);
-  float* scr = scratch + warp * kEpiScrFloats;
-  float s = 1.f;
-  if constexpr (!kRowwise) s = __ldg(scale_a) * scale_w;
-  int stage = 0;
-  uint32_t phase = 0;
-  for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-    const int m_blk = tile % num_m, n_blk = tile / num_m;
-    float acc[F8F_BN / 2];
-    gemm_mainloop<F8F_BN, 2, 1, false>(acc, a_base, b_base, F8_A_BYTES, F8F_B_BYTES, F8_STAGES, full_bar, empty_bar,
-                                       stage, phase, 0, num_k);
-    if constexpr (kRowwise)
-      gemm_frag_epilogue<F8F_BN, true, kEpi, true>(acc, scr, m_blk * F8_BM + wg * 64 + (warp & 3) * 16, n_blk * F8F_BN,
-                                                   F8F_BN, s, p, scale_a, scale_w);
-    else
-      gemm_frag_epilogue<F8F_BN, true, kEpi>(acc, scr, m_blk * F8_BM + wg * 64 + (warp & 3) * 16, n_blk * F8F_BN,
-                                             F8F_BN, s, p);
-  }
-}
-
-// Block scaling (torchao PerBlock [1, 128] activations / [128, 128] weights, the DeepSeek-V3 recipe): the promoted
-// kernel's structure and tile, with each k-block's partial multiplied by sa[kb][row] * sw[n_blk][kb] at the promotion
-// (gemm_mainloop<..., kBlockScale>).  The 128 x 128 tile spans exactly one weight block in N and one activation group
-// per k-block, so the epilogue applies no scale.  A kernel of its own for the reason given above the fast kernel.
-//   scale_a: fp32 [K/128, ld_sa] (k-block-major: one k-block's row scales are contiguous), scale_w: fp32 [N/128, K/128]
-template <int kEpi>
-__global__ void __launch_bounds__(F8_THREADS, 1)
-gemm_fp8_blockwise_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
-                          const GemmParams p, const float* __restrict__ scale_a, long ld_sa,
-                          const float* __restrict__ scale_w) {
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
-                                             ~static_cast<uintptr_t>(1023));
-  uint8_t* smem_a = smem;
-  uint8_t* smem_b = smem + F8_STAGES * F8_A_BYTES;
-  float* scratch = reinterpret_cast<float*>(smem + F8_STAGES * F8_STAGE_BYTES);
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + F8_STAGES * F8_STAGE_BYTES + F8_SCR_BYTES);
-  uint64_t* full_bar = bars;
-  uint64_t* empty_bar = bars + F8_STAGES;
-
-  const int warp = threadIdx.x >> 5;
-  const int num_m = (p.M + F8_BM - 1) / F8_BM, num_n = p.N / F8_BN, num_tiles = num_m * num_n;
-  const int num_k = (p.K + F8_BK - 1) / F8_BK;
-
-  if (threadIdx.x == 256) {
-    prefetch_tmap(&tmap_a);
-    prefetch_tmap(&tmap_b);
-    for (int i = 0; i < F8_STAGES; ++i) {
-      mbar_init(&full_bar[i], 1);
-      mbar_init(&empty_bar[i], 2);
-    }
-    fence_barrier_init();
-  }
-  __syncthreads();
-
-  if (warp >= 8) {
-    producer_regs();
-    if (warp == 8 && elect_one()) {
-      int stage = 0;
-      uint32_t phase = 0;
-      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-        const int m_blk = tile % num_m, n_blk = tile / num_m;
-        for (int kb = 0; kb < num_k; ++kb) {
-          mbar_wait(&empty_bar[stage], phase ^ 1);
-          mbar_expect_tx(&full_bar[stage], F8_STAGE_BYTES);
-          tma_load_2d(smem_a + stage * F8_A_BYTES, &tmap_a, &full_bar[stage], kb * F8_BK, m_blk * F8_BM);
-          tma_load_2d(smem_b + stage * F8_B_BYTES, &tmap_b, &full_bar[stage], kb * F8_BK, n_blk * F8_BN);
-          if (++stage == F8_STAGES) {
-            stage = 0;
-            phase ^= 1;
-          }
-        }
-      }
-    }
-    return;
-  }
-  consumer_regs();
-  const int wg = warp >> 2, lane = threadIdx.x & 31;
-  const uint32_t a_base = smem_u32(smem_a) + wg * 64 * F8_BK, b_base = smem_u32(smem_b);
-  float* scr = scratch + warp * kEpiScrFloats;
-  int stage = 0;
-  uint32_t phase = 0;
-  for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-    const int m_blk = tile % num_m, n_blk = tile / num_m;
-    const int row0 = m_blk * F8_BM + wg * 64 + (warp & 3) * 16;
-    const int r = row0 + (lane >> 2);
-    BlockScales bs;
-    bs.sa0 = r < p.M ? scale_a + r : nullptr;
-    bs.sa1 = r + 8 < p.M ? scale_a + r + 8 : nullptr;
-    bs.ld = ld_sa;
-    bs.sw = scale_w + static_cast<long>(n_blk) * num_k;
-    float acc[F8_BN / 2];
-    gemm_mainloop<F8_BN, 2, 1, true, true>(acc, a_base, b_base, F8_A_BYTES, F8_B_BYTES, F8_STAGES, full_bar,
-                                           empty_bar, stage, phase, 0, num_k, bs);
-    gemm_frag_epilogue<F8_BN, true, kEpi>(acc, scr, row0, n_blk * F8_BN, F8_BN, 1.f, p);
   }
 }
 
@@ -355,10 +220,11 @@ int fp8_quantize(const void* x, long ld, int rows, int cols, void* q, long ldq, 
 // ---------------------------------------------------------------------------
 // host launcher
 // ---------------------------------------------------------------------------
-template <bool kFast, int kEpi, bool kRowwise>
-static int launch_fp8(const void* a, int lda, const void* w, int ldw, const GemmParams& p, const float* scale_a,
-                      typename Fp8ScaleW<kRowwise>::type scale_w, cudaStream_t stream) {
-  constexpr int BN = kFast ? F8F_BN : F8_BN, SMEM = kFast ? F8F_SMEM : F8_SMEM;
+template <bool kFast, int kEpi, int kScale, typename... ScaleW>
+static int launch_fp8(const void* a, int lda, const void* w, int ldw, const GemmParams& p, cudaStream_t stream,
+                      const float* scale_a, ScaleW... scale_w) {
+  constexpr int BN = f8_bn(kFast), SMEM = f8_smem(kFast);
+  constexpr const char* name = kScale == F8_SCALE_BLOCK ? "gemm_fp8_blockwise" : "gemm_fp8";
   CUtensorMap ta, tb;
   // byte tensors: [rows, K] uint8, box [128 | 256 rows, 128 bytes], SWIZZLE_128B
   const uint64_t da[2] = {static_cast<uint64_t>(p.K), static_cast<uint64_t>(p.M)};
@@ -371,12 +237,12 @@ static int launch_fp8(const void* a, int lda, const void* w, int ldw, const Gemm
   const uint32_t bb[2] = {F8_BK, BN};
   rc = make_tmap_u8(&tb, w, 2, db, sb, bb, 128);
   if (rc != KR_OK) return rc;
-  auto kern = kFast ? gemm_fp8_fast_kernel<kEpi, kRowwise> : gemm_fp8_kernel<kEpi, kRowwise>;
+  const auto kern = gemm_fp8_kernel<kEpi, kScale, kFast, ScaleW...>;
   static bool attr_set = false;
   if (!attr_set) {
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM);
     if (e != cudaSuccess) {
-      set_last_error("gemm_fp8: cudaFuncSetAttribute failed: %s", cudaGetErrorString(e));
+      set_last_error("%s: cudaFuncSetAttribute failed: %s", name, cudaGetErrorString(e));
       return KR_ERR_CUDA;
     }
     attr_set = true;
@@ -384,148 +250,94 @@ static int launch_fp8(const void* a, int lda, const void* w, int ldw, const Gemm
   const int num_tiles = ((p.M + F8_BM - 1) / F8_BM) * (p.N / BN);
   int grid = sm_count();
   if (grid > num_tiles) grid = num_tiles;
-  kern<<<grid, F8_THREADS, SMEM, stream>>>(ta, tb, p, scale_a, scale_w);
+  kern<<<grid, F8_THREADS, SMEM, stream>>>(ta, tb, p, scale_a, scale_w...);
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) {
-    set_last_error("gemm_fp8: launch failed: %s", cudaGetErrorString(e));
+    set_last_error("%s: launch failed: %s", name, cudaGetErrorString(e));
     return KR_ERR_CUDA;
   }
   return KR_OK;
 }
 
-static int check_fp8(const char* who, int bn, int epi, int lda, int ldw, const GemmParams& p) {
-  if (p.M <= 0 || p.N <= 0 || p.K <= 0 || p.N % bn != 0 || p.K % 16 != 0 || lda % 16 != 0 || ldw % 16 != 0 ||
-      p.ldc % 8 != 0) {
+// The argument checks of every mode, then the kernel of the epilogue (EPI_F32 only with block scales).
+template <bool kFast, int kScale, typename... ScaleW>
+static int gemm_fp8_any(const char* who, int epi, const void* a, int lda, const void* w, int ldw, const GemmParams& p,
+                        cudaStream_t stream, const float* scale_a, ScaleW... scale_w) {
+  if (p.M <= 0 || p.N <= 0 || p.K <= 0 || p.N % f8_bn(kFast) != 0 || p.K % 16 != 0 || lda % 16 != 0 ||
+      ldw % 16 != 0 || p.ldc % 8 != 0) {
     set_last_error("%s: unsupported shape M=%d N=%d K=%d (need N %% %d == 0, K / ld %% 16 == 0)", who, p.M, p.N, p.K,
-                   bn);
+                   f8_bn(kFast));
     return KR_ERR_UNSUPPORTED_SHAPE;
   }
   if ((epi == EPI_BIAS_GATE_RES || epi == EPI_BIAS_RES || epi == EPI_MUL) && p.residual == nullptr) {
     set_last_error("%s: residual epilogue without residual pointer", who);
     return KR_ERR_INVALID_ARG;
   }
-  return KR_OK;
-}
-
-template <bool kFast>
-static int gemm_fp8_any(const char* who, int epi, const void* a, int lda, const void* w, int ldw, const GemmParams& p,
-                        const float* scale_a, float scale_w, cudaStream_t stream) {
-  const int rc = check_fp8(who, kFast ? F8F_BN : F8_BN, epi, lda, ldw, p);
-  if (rc != KR_OK) return rc;
-  if (scale_a == nullptr) {
-    set_last_error("%s: null activation scale", who);
-    return KR_ERR_INVALID_ARG;
+  if constexpr (kScale == F8_SCALE_TENSOR) {
+    if (scale_a == nullptr) {
+      set_last_error("%s: null activation scale", who);
+      return KR_ERR_INVALID_ARG;
+    }
+  } else if constexpr (kScale == F8_SCALE_ROW) {
+    const float* sw = f8_arg<0>(scale_w...);
+    if (scale_a == nullptr || sw == nullptr) {
+      set_last_error("%s: null row or channel scales", who);
+      return KR_ERR_INVALID_ARG;
+    }
+    if (reinterpret_cast<uintptr_t>(sw) % 16 != 0) {
+      set_last_error("%s: channel scales must be 16-byte aligned", who);
+      return KR_ERR_INVALID_ARG;
+    }
+  } else {
+    // the host-side checks of kr_api.cu (shape, pitches, null scales) have passed; these guard direct callers
+    if (p.K % F8_BK != 0) {
+      set_last_error("%s: K=%d is not a multiple of the 128-wide scale block", who, p.K);
+      return KR_ERR_UNSUPPORTED_SHAPE;
+    }
+    const long ld_sa = f8_arg<0>(scale_w...);
+    if (scale_a == nullptr || f8_arg<1>(scale_w...) == nullptr || ld_sa < p.M) {
+      set_last_error("%s: null block scales or activation scale pitch %ld < M=%d", who, ld_sa, p.M);
+      return KR_ERR_INVALID_ARG;
+    }
   }
   switch (epi) {
-    case EPI_BIAS: return launch_fp8<kFast, EPI_BIAS, false>(a, lda, w, ldw, p, scale_a, scale_w, stream);
-    case EPI_BIAS_GELU: return launch_fp8<kFast, EPI_BIAS_GELU, false>(a, lda, w, ldw, p, scale_a, scale_w, stream);
-    case EPI_BIAS_GATE_RES: return launch_fp8<kFast, EPI_BIAS_GATE_RES, false>(a, lda, w, ldw, p, scale_a, scale_w, stream);
-    case EPI_BIAS_RES: return launch_fp8<kFast, EPI_BIAS_RES, false>(a, lda, w, ldw, p, scale_a, scale_w, stream);
-    default: set_last_error("%s: unsupported epilogue %d", who, epi); return KR_ERR_INVALID_ARG;
-  }
-}
-
-template <bool kFast>
-static int gemm_fp8_rowwise_any(const char* who, int epi, const void* a, int lda, const void* w, int ldw,
-                                const GemmParams& p, const float* scale_a, const float* scale_w, cudaStream_t stream) {
-  const int rc = check_fp8(who, kFast ? F8F_BN : F8_BN, epi, lda, ldw, p);
-  if (rc != KR_OK) return rc;
-  if (scale_a == nullptr || scale_w == nullptr) {
-    set_last_error("%s: null row or channel scales", who);
-    return KR_ERR_INVALID_ARG;
-  }
-  if (reinterpret_cast<uintptr_t>(scale_w) % 16 != 0) {
-    set_last_error("%s: channel scales must be 16-byte aligned", who);
-    return KR_ERR_INVALID_ARG;
-  }
-  switch (epi) {
-    case EPI_BIAS: return launch_fp8<kFast, EPI_BIAS, true>(a, lda, w, ldw, p, scale_a, scale_w, stream);
-    case EPI_BIAS_GELU: return launch_fp8<kFast, EPI_BIAS_GELU, true>(a, lda, w, ldw, p, scale_a, scale_w, stream);
-    case EPI_BIAS_GATE_RES: return launch_fp8<kFast, EPI_BIAS_GATE_RES, true>(a, lda, w, ldw, p, scale_a, scale_w, stream);
-    case EPI_BIAS_RES: return launch_fp8<kFast, EPI_BIAS_RES, true>(a, lda, w, ldw, p, scale_a, scale_w, stream);
+    case EPI_BIAS: return launch_fp8<kFast, EPI_BIAS, kScale>(a, lda, w, ldw, p, stream, scale_a, scale_w...);
+    case EPI_BIAS_GELU: return launch_fp8<kFast, EPI_BIAS_GELU, kScale>(a, lda, w, ldw, p, stream, scale_a, scale_w...);
+    case EPI_BIAS_GATE_RES:
+      return launch_fp8<kFast, EPI_BIAS_GATE_RES, kScale>(a, lda, w, ldw, p, stream, scale_a, scale_w...);
+    case EPI_BIAS_RES: return launch_fp8<kFast, EPI_BIAS_RES, kScale>(a, lda, w, ldw, p, stream, scale_a, scale_w...);
+    case EPI_F32:
+      if constexpr (kScale == F8_SCALE_BLOCK)
+        return launch_fp8<kFast, EPI_F32, kScale>(a, lda, w, ldw, p, stream, scale_a, scale_w...);
+      [[fallthrough]];
     default: set_last_error("%s: unsupported epilogue %d", who, epi); return KR_ERR_INVALID_ARG;
   }
 }
 
 int gemm_fp8_tn(int epi, const void* a, int lda, const void* w, int ldw, const GemmParams& p, const float* scale_a,
                 float scale_w, cudaStream_t stream) {
-  return gemm_fp8_any<false>("gemm_fp8", epi, a, lda, w, ldw, p, scale_a, scale_w, stream);
+  return gemm_fp8_any<false, F8_SCALE_TENSOR>("gemm_fp8", epi, a, lda, w, ldw, p, stream, scale_a, scale_w);
 }
 
 int gemm_fp8_rowwise_tn(int epi, const void* a, int lda, const void* w, int ldw, const GemmParams& p,
                         const float* scale_a, const float* scale_w, cudaStream_t stream) {
-  return gemm_fp8_rowwise_any<false>("gemm_fp8_rowwise", epi, a, lda, w, ldw, p, scale_a, scale_w, stream);
+  return gemm_fp8_any<false, F8_SCALE_ROW>("gemm_fp8_rowwise", epi, a, lda, w, ldw, p, stream, scale_a, scale_w);
 }
 
 int gemm_fp8_fast_tn(int epi, const void* a, int lda, const void* w, int ldw, const GemmParams& p,
                      const float* scale_a, float scale_w, cudaStream_t stream) {
-  return gemm_fp8_any<true>("gemm_fp8_fast", epi, a, lda, w, ldw, p, scale_a, scale_w, stream);
+  return gemm_fp8_any<true, F8_SCALE_TENSOR>("gemm_fp8_fast", epi, a, lda, w, ldw, p, stream, scale_a, scale_w);
 }
 
 int gemm_fp8_rowwise_fast_tn(int epi, const void* a, int lda, const void* w, int ldw, const GemmParams& p,
                              const float* scale_a, const float* scale_w, cudaStream_t stream) {
-  return gemm_fp8_rowwise_any<true>("gemm_fp8_rowwise_fast", epi, a, lda, w, ldw, p, scale_a, scale_w, stream);
-}
-
-template <int kEpi>
-static int launch_fp8_blockwise(const void* a, int lda, const void* w, int ldw, const GemmParams& p,
-                                const float* scale_a, long ld_sa, const float* scale_w, cudaStream_t stream) {
-  CUtensorMap ta, tb;
-  const uint64_t da[2] = {static_cast<uint64_t>(p.K), static_cast<uint64_t>(p.M)};
-  const uint64_t sa[1] = {static_cast<uint64_t>(lda)};
-  const uint32_t ba[2] = {F8_BK, F8_BM};
-  int rc = make_tmap_u8(&ta, a, 2, da, sa, ba, 128);
-  if (rc != KR_OK) return rc;
-  const uint64_t db[2] = {static_cast<uint64_t>(p.K), static_cast<uint64_t>(p.N)};
-  const uint64_t sb[1] = {static_cast<uint64_t>(ldw)};
-  const uint32_t bb[2] = {F8_BK, F8_BN};
-  rc = make_tmap_u8(&tb, w, 2, db, sb, bb, 128);
-  if (rc != KR_OK) return rc;
-  static bool attr_set = false;
-  if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(gemm_fp8_blockwise_kernel<kEpi>,
-                                         cudaFuncAttributeMaxDynamicSharedMemorySize, F8_SMEM);
-    if (e != cudaSuccess) {
-      set_last_error("gemm_fp8_blockwise: cudaFuncSetAttribute failed: %s", cudaGetErrorString(e));
-      return KR_ERR_CUDA;
-    }
-    attr_set = true;
-  }
-  const int num_tiles = ((p.M + F8_BM - 1) / F8_BM) * (p.N / F8_BN);
-  int grid = sm_count();
-  if (grid > num_tiles) grid = num_tiles;
-  gemm_fp8_blockwise_kernel<kEpi><<<grid, F8_THREADS, F8_SMEM, stream>>>(ta, tb, p, scale_a, ld_sa, scale_w);
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) {
-    set_last_error("gemm_fp8_blockwise: launch failed: %s", cudaGetErrorString(e));
-    return KR_ERR_CUDA;
-  }
-  return KR_OK;
+  return gemm_fp8_any<true, F8_SCALE_ROW>("gemm_fp8_rowwise_fast", epi, a, lda, w, ldw, p, stream, scale_a, scale_w);
 }
 
 int gemm_fp8_blockwise_tn(int epi, const void* a, int lda, const void* w, int ldw, const GemmParams& p,
                           const float* scale_a, int ld_sa, const float* scale_w, cudaStream_t stream) {
-  // the host-side checks of kr_api.cu (shape, pitches, null scales) have passed; these guard direct callers
-  const char* who = "gemm_fp8_blockwise";
-  int rc = check_fp8(who, F8_BN, epi, lda, ldw, p);
-  if (rc != KR_OK) return rc;
-  if (p.K % F8_BK != 0) {
-    set_last_error("%s: K=%d is not a multiple of the 128-wide scale block", who, p.K);
-    return KR_ERR_UNSUPPORTED_SHAPE;
-  }
-  if (scale_a == nullptr || scale_w == nullptr || ld_sa < p.M) {
-    set_last_error("%s: null block scales or activation scale pitch %d < M=%d", who, ld_sa, p.M);
-    return KR_ERR_INVALID_ARG;
-  }
-  switch (epi) {
-    case EPI_BIAS: return launch_fp8_blockwise<EPI_BIAS>(a, lda, w, ldw, p, scale_a, ld_sa, scale_w, stream);
-    case EPI_BIAS_GELU: return launch_fp8_blockwise<EPI_BIAS_GELU>(a, lda, w, ldw, p, scale_a, ld_sa, scale_w, stream);
-    case EPI_BIAS_GATE_RES:
-      return launch_fp8_blockwise<EPI_BIAS_GATE_RES>(a, lda, w, ldw, p, scale_a, ld_sa, scale_w, stream);
-    case EPI_BIAS_RES: return launch_fp8_blockwise<EPI_BIAS_RES>(a, lda, w, ldw, p, scale_a, ld_sa, scale_w, stream);
-    case EPI_F32: return launch_fp8_blockwise<EPI_F32>(a, lda, w, ldw, p, scale_a, ld_sa, scale_w, stream);
-    default: set_last_error("%s: unsupported epilogue %d", who, epi); return KR_ERR_INVALID_ARG;
-  }
+  return gemm_fp8_any<false, F8_SCALE_BLOCK>("gemm_fp8_blockwise", epi, a, lda, w, ldw, p, stream, scale_a,
+                                             static_cast<long>(ld_sa), scale_w);
 }
 
 }  // namespace kr

@@ -246,6 +246,29 @@ def dit_block_fwd(x: torch.Tensor, e0: torch.Tensor, modulation: torch.Tensor, r
 _fp8_scratch = {}
 
 
+def _fp8_cast_scratch(kind: str, x: torch.Tensor):
+    """``x`` as [rows, cols] and the (q, scale) buffers its ``kind`` ("tensor", "rows" or "blocks") FP8 cast writes,
+    reused per (kind, device, rows, cols); the launches are stream-ordered."""
+    rows, _ = _rows2d(x, "x")
+    cols = x.shape[-1]
+    key = (kind, x.device.index, rows, cols)
+    sc = _fp8_scratch.get(key)
+    if sc is None:
+        scale_shape = {"tensor": (2,), "rows": (rows,), "blocks": (cols // 128, rows)}[kind]
+        sc = _fp8_scratch[key] = (torch.empty(rows, cols, dtype=torch.uint8, device=x.device),
+                                  torch.empty(scale_shape, dtype=torch.float32, device=x.device))
+    return (x if x.dim() == 2 else x.reshape(rows, -1)), *sc
+
+
+def _fp8_epi_pitches(out: torch.Tensor, residual, gate, out2):
+    """Row pitches of an FP8 GEMM's epilogue tensors: (ldc, ldr, gate stride, ldc2), 0 for an absent one."""
+    _, ldc = _rows2d(out, "out")
+    ldr = _rows2d(residual, "residual")[1] if residual is not None else 0
+    gs = gate.stride(0) if gate is not None and gate.dim() >= 2 else 0
+    ldc2 = _rows2d(out2, "out2")[1] if out2 is not None else 0
+    return ldc, ldr, gs, ldc2
+
+
 def fp8_quantize(x: torch.Tensor, q: Optional[torch.Tensor] = None, state: Optional[torch.Tensor] = None):
     """Dynamic per-tensor e4m3 cast (torchao Float8DynamicActivation, PerTensor): x [rows, cols] bf16 ->
     (q uint8 bytes [rows, cols], state float32 [2] = [amax, dequantisation scale amax / 448])."""
@@ -276,10 +299,7 @@ def gemm_fp8(a_q: torch.Tensor, w_q: torch.Tensor, scale_a: torch.Tensor, scale_
     N = w_q.shape[0]
     if out is None:
         out = torch.empty(M, N, dtype=torch.bfloat16, device=a_q.device)
-    _, ldc = _rows2d(out, "out")
-    ldr = _rows2d(residual, "residual")[1] if residual is not None else 0
-    gs = gate.stride(0) if gate is not None and gate.dim() >= 2 else 0
-    ldc2 = _rows2d(out2, "out2")[1] if out2 is not None else 0
+    ldc, ldr, gs, ldc2 = _fp8_epi_pitches(out, residual, gate, out2)
     lib = _lib.load()
     name = "kr_gemm_fp8_fast" if fast_accum else "kr_gemm_fp8"
     with _Timed("gemm_fp8_fast" if fast_accum else "gemm_fp8", 2.0 * M * N * K):
@@ -295,13 +315,7 @@ def gemm_fp8(a_q: torch.Tensor, w_q: torch.Tensor, scale_a: torch.Tensor, scale_
 def linear_fp8(x: torch.Tensor, w_q: torch.Tensor, scale_w: float, bias: Optional[torch.Tensor] = None, **kw):
     """Float8 dynamic-activation linear: quantise ``x`` per tensor, then the FP8 GEMM (scratch buffers are reused per
     (device, shape); the launches are stream-ordered)."""
-    rows, _ = _rows2d(x, "x")
-    key = (x.device.index, rows, x.shape[-1])
-    sc = _fp8_scratch.get(key)
-    if sc is None:
-        sc = _fp8_scratch[key] = (torch.empty(rows, x.shape[-1], dtype=torch.uint8, device=x.device),
-                                  torch.empty(2, dtype=torch.float32, device=x.device))
-    q, state = fp8_quantize(x if x.dim() == 2 else x.reshape(rows, -1), sc[0], sc[1])
+    q, state = fp8_quantize(*_fp8_cast_scratch("tensor", x))
     return gemm_fp8(q, w_q, state, scale_w, bias, **kw)
 
 
@@ -354,27 +368,8 @@ def ln_modulate_fp8(x: torch.Tensor, *, eps: float, weight: Optional[torch.Tenso
                     scale: Optional[torch.Tensor] = None) -> Fp8Rows:
     """:func:`ln_modulate` whose output rows are cast to e4m3 per row in the same kernel (exactly
     :func:`fp8_quantize_rows` of the bf16 output).  The bf16 output is written only when ``out`` is given."""
-    _req(x, "x", torch.bfloat16)
-    rows, ldx = _rows2d(x, "x")
-    D = x.shape[-1]
-    ldo = 0
-    if out is not None:
-        _req(out, "out", torch.bfloat16)
-        _, ldo = _rows2d(out, "out")
-    mod_rows = 0
-    if mod is not None:
-        _req(mod, "mod", torch.bfloat16)
-        if not mod.is_contiguous() or mod.shape[-1] != D:
-            raise _lib.KreaB200Error("ln_modulate_fp8: mod must be contiguous [frames, rows, D]")
-        mod_rows = mod.shape[-2]
-    q, scale = _rows_out(rows, D, x.device, q, scale)
-    lib = _lib.load()
-    rc = lib.kr_ln_modulate_fp8(x.data_ptr(), ldx, _ptr(out), ldo, rows, D, eps, _ptr(weight), _ptr(bias), _ptr(mod),
-                                mod_rows, shift_idx, scale_idx, rows_per_frame, row_offset, q.data_ptr(), q.stride(0),
-                                scale.data_ptr(), _stream())
-    _lib.check(rc, "kr_ln_modulate_fp8")
-    _count()
-    return Fp8Rows(q, scale, x.dtype)
+    return _ln_modulate_fp8(False, x, eps, weight, bias, mod, shift_idx, scale_idx, rows_per_frame, out, row_offset,
+                            q, scale)
 
 
 def gemm_fp8_rowwise(a: Fp8Rows, w_q: torch.Tensor, scale_w: torch.Tensor, bias: Optional[torch.Tensor] = None, *,
@@ -394,10 +389,7 @@ def gemm_fp8_rowwise(a: Fp8Rows, w_q: torch.Tensor, scale_w: torch.Tensor, bias:
                                  f"a.scale {tuple(a.scale.shape)} do not match M={M} K={K}")
     if out is None:
         out = torch.empty(M, N, dtype=torch.bfloat16, device=a.q.device)
-    _, ldc = _rows2d(out, "out")
-    ldr = _rows2d(residual, "residual")[1] if residual is not None else 0
-    gs = gate.stride(0) if gate is not None and gate.dim() >= 2 else 0
-    ldc2 = _rows2d(out2, "out2")[1] if out2 is not None else 0
+    ldc, ldr, gs, ldc2 = _fp8_epi_pitches(out, residual, gate, out2)
     lib = _lib.load()
     name = "kr_gemm_fp8_rowwise_fast" if fast_accum else "kr_gemm_fp8_rowwise"
     with _Timed("gemm_fp8_fast" if fast_accum else "gemm_fp8", 2.0 * M * N * K, sub="rowwise"):
@@ -410,21 +402,12 @@ def gemm_fp8_rowwise(a: Fp8Rows, w_q: torch.Tensor, scale_w: torch.Tensor, bias:
     return out
 
 
-_fp8_rows_scratch = {}
-
-
 def linear_fp8_rowwise(x, w_q: torch.Tensor, scale_w: torch.Tensor, bias: Optional[torch.Tensor] = None, **kw):
     """Float8 dynamic-activation linear with PerRow granularity: ``x`` is a bf16 activation (cast per row here, into
     scratch reused per (device, rows, cols); the launches are stream-ordered) or an :class:`Fp8Rows` already cast by
     :func:`ln_modulate_fp8` / :func:`fp8_quantize_rows`; then the row-scaled FP8 GEMM."""
     if not isinstance(x, Fp8Rows):
-        rows, _ = _rows2d(x, "x")
-        key = (x.device.index, rows, x.shape[-1])
-        sc = _fp8_rows_scratch.get(key)
-        if sc is None:
-            sc = _fp8_rows_scratch[key] = (torch.empty(rows, x.shape[-1], dtype=torch.uint8, device=x.device),
-                                           torch.empty(rows, dtype=torch.float32, device=x.device))
-        x = fp8_quantize_rows(x if x.dim() == 2 else x.reshape(rows, -1), sc[0], sc[1])
+        x = fp8_quantize_rows(*_fp8_cast_scratch("rows", x))
     return gemm_fp8_rowwise(x, w_q, scale_w, bias, **kw)
 
 
@@ -460,6 +443,34 @@ def _blocks_out(rows: int, cols: int, device, q: Optional[torch.Tensor], scale: 
     return q, scale
 
 
+def _ln_modulate_fp8(blocks: bool, x: torch.Tensor, eps: float, weight, bias, mod, shift_idx: int, scale_idx: int,
+                     rows_per_frame: int, out, row_offset: int, q, scale):
+    """The body of :func:`ln_modulate_fp8` (per-row cast) and :func:`ln_modulate_fp8_blocks` (per-group cast)."""
+    name = "ln_modulate_fp8_blocks" if blocks else "ln_modulate_fp8"
+    _req(x, "x", torch.bfloat16)
+    rows, ldx = _rows2d(x, "x")
+    D = x.shape[-1]
+    ldo = 0
+    if out is not None:
+        _req(out, "out", torch.bfloat16)
+        _, ldo = _rows2d(out, "out")
+    mod_rows = 0
+    if mod is not None:
+        _req(mod, "mod", torch.bfloat16)
+        if not mod.is_contiguous() or mod.shape[-1] != D:
+            raise _lib.KreaB200Error(f"{name}: mod must be contiguous [frames, rows, D]")
+        mod_rows = mod.shape[-2]
+    q, scale = (_blocks_out if blocks else _rows_out)(rows, D, x.device, q, scale)
+    ld_s = (scale.stride(0),) if blocks else ()
+    lib = _lib.load()
+    rc = getattr(lib, "kr_" + name)(x.data_ptr(), ldx, _ptr(out), ldo, rows, D, eps, _ptr(weight), _ptr(bias),
+                                    _ptr(mod), mod_rows, shift_idx, scale_idx, rows_per_frame, row_offset,
+                                    q.data_ptr(), q.stride(0), scale.data_ptr(), *ld_s, _stream())
+    _lib.check(rc, "kr_" + name)
+    _count()
+    return (Fp8Blocks if blocks else Fp8Rows)(q, scale, x.dtype)
+
+
 def fp8_quantize_blocks(x: torch.Tensor, q: Optional[torch.Tensor] = None,
                         scale: Optional[torch.Tensor] = None) -> Fp8Blocks:
     """Dynamic per-group e4m3 cast (torchao PerBlock [1, 128]): x [rows, cols] bf16 (row pitch free, cols % 128 == 0)
@@ -483,27 +494,8 @@ def ln_modulate_fp8_blocks(x: torch.Tensor, *, eps: float, weight: Optional[torc
                            scale: Optional[torch.Tensor] = None) -> Fp8Blocks:
     """:func:`ln_modulate` whose output rows are cast to e4m3 per 128-channel group in the same kernel (exactly
     :func:`fp8_quantize_blocks` of the bf16 output).  The bf16 output is written only when ``out`` is given."""
-    _req(x, "x", torch.bfloat16)
-    rows, ldx = _rows2d(x, "x")
-    D = x.shape[-1]
-    ldo = 0
-    if out is not None:
-        _req(out, "out", torch.bfloat16)
-        _, ldo = _rows2d(out, "out")
-    mod_rows = 0
-    if mod is not None:
-        _req(mod, "mod", torch.bfloat16)
-        if not mod.is_contiguous() or mod.shape[-1] != D:
-            raise _lib.KreaB200Error("ln_modulate_fp8_blocks: mod must be contiguous [frames, rows, D]")
-        mod_rows = mod.shape[-2]
-    q, scale = _blocks_out(rows, D, x.device, q, scale)
-    lib = _lib.load()
-    rc = lib.kr_ln_modulate_fp8_blocks(x.data_ptr(), ldx, _ptr(out), ldo, rows, D, eps, _ptr(weight), _ptr(bias),
-                                       _ptr(mod), mod_rows, shift_idx, scale_idx, rows_per_frame, row_offset,
-                                       q.data_ptr(), q.stride(0), scale.data_ptr(), scale.stride(0), _stream())
-    _lib.check(rc, "kr_ln_modulate_fp8_blocks")
-    _count()
-    return Fp8Blocks(q, scale, x.dtype)
+    return _ln_modulate_fp8(True, x, eps, weight, bias, mod, shift_idx, scale_idx, rows_per_frame, out, row_offset,
+                            q, scale)
 
 
 def gemm_fp8_blockwise(a: Fp8Blocks, w_q: torch.Tensor, scale_w: torch.Tensor, bias: Optional[torch.Tensor] = None,
@@ -525,10 +517,7 @@ def gemm_fp8_blockwise(a: Fp8Blocks, w_q: torch.Tensor, scale_w: torch.Tensor, b
                                  f"a.scale {tuple(a.scale.shape)} do not match M={M} K={K}")
     if out is None:
         out = torch.empty(M, N, dtype=torch.float32 if epilogue == EPI_F32 else torch.bfloat16, device=a.q.device)
-    _, ldc = _rows2d(out, "out")
-    ldr = _rows2d(residual, "residual")[1] if residual is not None else 0
-    gs = gate.stride(0) if gate is not None and gate.dim() >= 2 else 0
-    ldc2 = _rows2d(out2, "out2")[1] if out2 is not None else 0
+    ldc, ldr, gs, ldc2 = _fp8_epi_pitches(out, residual, gate, out2)
     lib = _lib.load()
     with _Timed("gemm_fp8", 2.0 * M * N * K, sub="blockwise"):
         rc = lib.kr_gemm_fp8_blockwise(epilogue, a.q.data_ptr(), a.q.stride(0), w_q.data_ptr(), w_q.stride(0),
@@ -540,23 +529,13 @@ def gemm_fp8_blockwise(a: Fp8Blocks, w_q: torch.Tensor, scale_w: torch.Tensor, b
     return out
 
 
-_fp8_blocks_scratch = {}
-
-
 def linear_fp8_blockwise(x, w_q: torch.Tensor, scale_w: torch.Tensor, bias: Optional[torch.Tensor] = None, **kw):
     """Float8 dynamic-activation linear with PerBlock granularity: ``x`` is a bf16 activation (cast per 128-channel
     group here, into scratch reused per (device, rows, cols); the launches are stream-ordered) or an
     :class:`Fp8Blocks` already cast by :func:`ln_modulate_fp8_blocks` / :func:`fp8_quantize_blocks`; then the
     block-scaled FP8 GEMM."""
     if not isinstance(x, Fp8Blocks):
-        rows, _ = _rows2d(x, "x")
-        key = (x.device.index, rows, x.shape[-1])
-        sc = _fp8_blocks_scratch.get(key)
-        if sc is None:
-            sc = _fp8_blocks_scratch[key] = (
-                torch.empty(rows, x.shape[-1], dtype=torch.uint8, device=x.device),
-                torch.empty(x.shape[-1] // 128, rows, dtype=torch.float32, device=x.device))
-        x = fp8_quantize_blocks(x if x.dim() == 2 else x.reshape(rows, -1), sc[0], sc[1])
+        x = fp8_quantize_blocks(*_fp8_cast_scratch("blocks", x))
     return gemm_fp8_blockwise(x, w_q, scale_w, bias, **kw)
 
 

@@ -14,7 +14,7 @@ import torch
 
 from oracle import fp8_blockwise_oracle as F8B
 from oracle import fp8_rowwise_oracle as F8R
-from tests import cpu_ops_emulation_fp8_blocks as emu
+from tests import cpu_ops_emulation_fp8 as emu
 from tests.golden_io import rel_l2
 from tests.test_fp8_rowwise_cpu import _run, _small_model
 
@@ -283,27 +283,11 @@ def test_argument_validation_of_the_block_fp8_entry_points(lib):
     assert gemm(0, s, s, ld_sa=100) == -1                    # activation scale pitch < M
 
 
-def _funcs_and_usage():
-    from realtime_video_b200 import _lib
-    from tests.test_fp8_rowwise_cpu import _resource_usage
-    _lib.load()
-    out = subprocess.run(["cuobjdump", "-sass", str(_lib.LIB_PATH)], capture_output=True, text=True, check=True).stdout
-    funcs, name = {}, None
-    for line in out.splitlines():
-        m = re.search(r"Function : (\S+)", line)
-        if m:
-            name = m.group(1)
-            funcs[name] = []
-        elif name and re.match(r"\s+/\*[0-9a-f]{4,}\*/", line):
-            funcs[name].append(line.split("*/", 1)[1].strip())
-    return funcs, _resource_usage()
-
-
 @pytest.mark.skipif(shutil.which("cuobjdump") is None, reason="cuobjdump not on PATH")
-def test_sass_and_resources_of_the_block_fp8_kernels():
-    from tests.test_sass_cpu import _ops
-    funcs, usage = _funcs_and_usage()
-    gemms = [f for f in funcs if "gemm_fp8_blockwise_kernel" in f]
+def test_sass_and_resources_of_the_block_scaled_gemm_instantiations():
+    from tests.test_sass_cpu import _ops, resource_usage, sass_functions
+    funcs, usage = sass_functions(), resource_usage()
+    gemms = [f for f in funcs if re.search(r"gemm_fp8_kernelILi\dELi2ELb0E", f)]   # block scales, promoted
     assert len(gemms) == 5                                   # bias, GELU, gate + residual, residual, fp32
     for f in gemms:
         ops = {o.split(".")[0] for o in _ops(funcs[f])}

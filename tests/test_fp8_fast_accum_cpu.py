@@ -11,7 +11,7 @@ from pathlib import Path
 import pytest
 import torch
 
-from tests import cpu_ops_emulation_fp8_fast as emu
+from tests import cpu_ops_emulation_fp8 as emu
 from tests.golden_io import load_npz, rel_l2, weights
 
 ROOT = Path(__file__).resolve().parent.parent
@@ -199,31 +199,16 @@ def test_fast_entry_points_are_exported_and_validate_their_arguments(lib):
     assert rows(scale_w=ctypes.c_void_p(8196)) == -1 and b"aligned" in lib.kr_last_error()
 
 
-def _cuobjdump(*args):
-    from realtime_video_b200 import _lib
-    _lib.load()
-    return subprocess.run(["cuobjdump", *args, str(_lib.LIB_PATH)], capture_output=True, text=True, check=True).stdout
-
-
 @pytest.mark.skipif(shutil.which("cuobjdump") is None, reason="cuobjdump not on PATH")
-def test_sass_and_resources_of_the_fast_kernel():
-    """gemm_fp8_fast_kernel is e4m3 wgmma (QGMMA) fed by TMA through mbarriers, in four epilogues for each scale mode,
+def test_sass_and_resources_of_the_fast_accum_gemm_instantiations():
+    """gemm_fp8_kernel<kFast = true> is e4m3 wgmma (QGMMA) fed by TMA through mbarriers, in four epilogues for each scale mode,
     for sm_90a only, without a legacy tensor-core path, stack or local memory, and within the 168 registers that 384
     threads per SM allow at launch (the consumers raise theirs to 232 with setmaxnreg)."""
-    from tests.test_sass_cpu import _ops
-    assert set(re.findall(r"sm_\d+a?", _cuobjdump("-lelf"))) == {"sm_90a"}
-    funcs, name = {}, None
-    for line in _cuobjdump("-sass").splitlines():
-        m = re.search(r"Function : (\S+)", line)
-        if m:
-            name = m.group(1)
-            funcs[name] = []
-        elif name and re.match(r"\s+/\*[0-9a-f]{4,}\*/", line):
-            funcs[name].append(line.split("*/", 1)[1].strip())
-    usage = {m.group(1): tuple(int(re.search(k + r":(\d+)", m.group(2)).group(1)) for k in ("REG", "STACK", "LOCAL"))
-             for m in re.finditer(r"Function (\S+):\s*\n\s*(.*)", _cuobjdump("--dump-resource-usage"))}
+    from tests.test_sass_cpu import _ops, cuobjdump, resource_usage, sass_functions
+    assert set(re.findall(r"sm_\d+a?", cuobjdump("-lelf"))) == {"sm_90a"}
+    funcs, usage = sass_functions(), resource_usage()
     for rowwise in (0, 1):
-        kern = [f for f in funcs if re.search(rf"gemm_fp8_fast_kernelILi\dELb{rowwise}E", f)]
+        kern = [f for f in funcs if re.search(rf"gemm_fp8_kernelILi\dELi{rowwise}ELb1E", f)]   # fast accumulation
         assert len(kern) == 4, kern                                 # bias, GELU, gate + residual, residual
         for f in kern:
             ops = _ops(funcs[f])

@@ -15,7 +15,7 @@ import torch
 
 from oracle import fp8_oracle as F8T
 from oracle import fp8_rowwise_oracle as F8
-from tests import cpu_ops_emulation_fp8_rows as emu
+from tests import cpu_ops_emulation_fp8 as emu
 from tests.golden_io import load_npz, rel_l2, weights
 
 ROOT = Path(__file__).resolve().parent.parent
@@ -270,39 +270,11 @@ def test_argument_validation_of_the_row_fp8_entry_points(lib):
     assert gemm(0, s, ctypes.c_void_p(8196)) == -1 and b"aligned" in lib.kr_last_error()
 
 
-def _resource_usage():
-    from realtime_video_b200 import _lib
-    _lib.load()
-    out = subprocess.run(["cuobjdump", "--dump-resource-usage", str(_lib.LIB_PATH)], capture_output=True, text=True,
-                         check=True).stdout
-    usage, name = {}, None
-    for line in out.splitlines():
-        m = re.search(r"Function (\S+):", line)
-        if m:
-            name = m.group(1)
-        elif name and "REG:" in line:
-            usage[name] = (int(re.search(r"REG:(\d+)", line).group(1)), int(re.search(r"STACK:(\d+)", line).group(1)),
-                           int(re.search(r"LOCAL:(\d+)", line).group(1)))
-            name = None
-    return usage
-
-
 @pytest.mark.skipif(shutil.which("cuobjdump") is None, reason="cuobjdump not on PATH")
-def test_sass_and_resources_of_the_row_fp8_kernels():
-    from tests.test_sass_cpu import _ops
-    from realtime_video_b200 import _lib
-    _lib.load()
-    out = subprocess.run(["cuobjdump", "-sass", str(_lib.LIB_PATH)], capture_output=True, text=True, check=True).stdout
-    funcs, name = {}, None
-    for line in out.splitlines():
-        m = re.search(r"Function : (\S+)", line)
-        if m:
-            name = m.group(1)
-            funcs[name] = []
-        elif name and re.match(r"\s+/\*[0-9a-f]{4,}\*/", line):
-            funcs[name].append(line.split("*/", 1)[1].strip())
-    usage = _resource_usage()
-    rowwise = [f for f in funcs if re.search(r"gemm_fp8_kernelILi\dELb1E", f)]
+def test_sass_and_resources_of_the_row_scaled_gemm_instantiations():
+    from tests.test_sass_cpu import _ops, resource_usage, sass_functions
+    funcs, usage = sass_functions(), resource_usage()
+    rowwise = [f for f in funcs if re.search(r"gemm_fp8_kernelILi\dELi1ELb0E", f)]   # row scales, promoted
     assert len(rowwise) == 4                                          # bias, GELU, gate + residual, residual
     for f in rowwise:
         ops = set(_ops(funcs[f]))

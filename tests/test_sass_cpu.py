@@ -13,12 +13,15 @@ from realtime_video_b200 import _lib
 pytestmark = pytest.mark.skipif(shutil.which("cuobjdump") is None, reason="cuobjdump not on PATH")
 
 
-@pytest.fixture(scope="module")
-def sass():
+def cuobjdump(*args):
     _lib.load()                      # builds the library if needed
-    out = subprocess.run(["cuobjdump", "-sass", str(_lib.LIB_PATH)], capture_output=True, text=True, check=True).stdout
+    return subprocess.run(["cuobjdump", *args, str(_lib.LIB_PATH)], capture_output=True, text=True, check=True).stdout
+
+
+def sass_functions():
+    """{mangled name: [instruction lines]} of every function in the library."""
     funcs, name, body = {}, None, []
-    for line in out.splitlines():
+    for line in cuobjdump("-sass").splitlines():
         m = re.search(r"Function : (\S+)", line)
         if m:
             if name:
@@ -31,13 +34,23 @@ def sass():
     return funcs
 
 
+def resource_usage():
+    """{mangled name: (REG, STACK, LOCAL)} of every function in the library."""
+    return {m.group(1): tuple(int(re.search(k + r":(\d+)", m.group(2)).group(1)) for k in ("REG", "STACK", "LOCAL"))
+            for m in re.finditer(r"Function (\S+):\s*\n\s*(.*)", cuobjdump("--dump-resource-usage"))}
+
+
+@pytest.fixture(scope="module")
+def sass():
+    return sass_functions()
+
+
 def _ops(body):
     return [(l.split()[1] if l.startswith("@") else l.split()[0]) for l in body if l]
 
 
 def test_compiled_for_sm_90a_only():
-    out = subprocess.run(["cuobjdump", "-lelf", str(_lib.LIB_PATH)], capture_output=True, text=True, check=True).stdout
-    archs = set(re.findall(r"sm_\d+a?", out))
+    archs = set(re.findall(r"sm_\d+a?", cuobjdump("-lelf")))
     assert archs == {"sm_90a"}, archs
 
 
@@ -79,19 +92,9 @@ def test_register_and_stack_budget():
     accumulators and epilogue in registers (no stack), the attention kernel stays within the 168 registers that
     384 threads per SM allow at launch (the consumer warpgroups raise theirs with setmaxnreg) with at most a few
     spill slots."""
-    out = subprocess.run(["cuobjdump", "--dump-resource-usage", str(_lib.LIB_PATH)], capture_output=True, text=True,
-                         check=True).stdout
-    usage = {}
-    name = None
-    for line in out.splitlines():
-        m = re.search(r"Function (\S+):", line)
-        if m:
-            name = m.group(1)
-        elif name and "REG:" in line:
-            usage[name] = (int(re.search(r"REG:(\d+)", line).group(1)), int(re.search(r"STACK:(\d+)", line).group(1)))
-            name = None
+    usage = resource_usage()
     assert usage
-    for fn, (reg, stack) in usage.items():
+    for fn, (reg, stack, _) in usage.items():
         head_conv = "conv_igemm_kernelILi96ELi16E" in fn      # 96 -> 3 head: runtime channel loop over a 16-entry array
         if any(k in fn for k in ("gemm_tn_kernel", "gemm_flex_kernel", "gemm2_tn_kernel", "conv_igemm_kernel",
                                  "conv_halo_kernel")) \
@@ -112,8 +115,6 @@ def test_jpeg_kernels_keep_their_tables_out_of_local_memory(sass):
     for name in ("jpeg_scan", "jpeg_stuff"):
         ops = next(v for k, v in kern.items() if name in k)
         assert any(o.startswith("SHFL.UP") for o in ops), name
-    out = subprocess.run(["cuobjdump", "--dump-resource-usage", str(_lib.LIB_PATH)], capture_output=True, text=True,
-                         check=True).stdout
-    for m in re.finditer(r"Function (\S*jpeg_\S*):\s*\n\s*(.*)", out):
-        stack = int(re.search(r"STACK:(\d+)", m.group(2)).group(1))
-        assert stack <= 16, (m.group(1), stack)               # a spilled temporary at most; no local arrays
+    for fn, (_, stack, _) in resource_usage().items():
+        if "jpeg_" in fn:
+            assert stack <= 16, (fn, stack)                   # a spilled temporary at most; no local arrays
