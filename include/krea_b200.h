@@ -328,5 +328,7 @@ int kr_rgb8_to_jpeg(const unsigned char* rgb, int frames, int height, int width,
 /* Block-scaled FP8 linears (kr_fp8_quantize_blocks / kr_ln_modulate_fp8_blocks / kr_gemm_fp8_blockwise): a header of
  * their own beside the PerTensor / PerRow entry points above; the API layer kr_api.cu defines them. */
 #include "krea_b200_fp8_blocks.h"
+/* INT8 linears (kr_i8_quantize_rows / kr_ln_modulate_i8 / kr_gemm_i8_rowwise): likewise, defined by kr_api.cu. */
+#include "krea_b200_int8.h"
 
 #endif /* KREA_B200_H_ */

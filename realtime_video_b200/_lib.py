@@ -186,6 +186,13 @@ FP8_BLOCK_SIGNATURES = {
                               _i, _i, _i, _vp],
 }
 
+# the INT8 linears (include/krea_b200_int8.h, kr_dit_elem.cu / kr_gemm_fp8.cu); every function returns int
+INT8_SIGNATURES = {
+    "kr_i8_quantize_rows": SIGNATURES["kr_fp8_quantize_rows"],
+    "kr_ln_modulate_i8": SIGNATURES["kr_ln_modulate_fp8"],
+    "kr_gemm_i8_rowwise": SIGNATURES["kr_gemm_fp8_rowwise"],
+}
+
 
 def load() -> ctypes.CDLL:
     """Load the shared library (building is the caller's job: ``__graft_entry__.build``)."""
@@ -212,7 +219,8 @@ def load() -> ctypes.CDLL:
         if hasattr(lib, "kr_jpeg_workspace_bytes"):
             lib.kr_jpeg_workspace_bytes.restype = _sz
             lib.kr_jpeg_workspace_bytes.argtypes = [_i, _i, _i]
-        for name, argtypes in {**SIGNATURES, **SAGE_SIGNATURES, **VAE_FP8_SIGNATURES, **FP8_BLOCK_SIGNATURES}.items():
+        for name, argtypes in {**SIGNATURES, **SAGE_SIGNATURES, **VAE_FP8_SIGNATURES, **FP8_BLOCK_SIGNATURES,
+                                **INT8_SIGNATURES}.items():
             fn = getattr(lib, name, None)
             if fn is None:
                 continue   # checked by tests/test_abi.py against the header

@@ -183,6 +183,38 @@ int kr_gemm_fp8_blockwise(int epilogue, const void* a, int lda, const void* w, i
                                    static_cast<cudaStream_t>(stream));
 }
 
+// INT8 linears (include/krea_b200_int8.h)
+int kr_i8_quantize_rows(const void* x, int ldx, int rows, int cols, void* q, int ldq, float* scale_rows,
+                        void* stream) {
+  KR_REQUIRE(x && q && scale_rows, "null x/q/scale_rows");
+  KR_REQUIRE_LINKED(i8_quantize_rows);
+  return kr::i8_quantize_rows(x, ldx, rows, cols, q, ldq, scale_rows, static_cast<cudaStream_t>(stream));
+}
+
+int kr_ln_modulate_i8(const void* x, int ldx, void* out, int ldo, int rows, int D, float eps,
+                      const void* w, const void* b, const void* mod, int mod_rows, int shift_idx,
+                      int scale_idx, int rows_per_frame, int row_offset, void* q, int ldq, float* scale_rows,
+                      void* stream) {
+  KR_REQUIRE(x && q && scale_rows, "null x/q/scale_rows");
+  KR_REQUIRE_LINKED(ln_modulate_i8);
+  return kr::ln_modulate_i8(x, ldx, out, ldo, rows, D, eps, w, b, mod, mod_rows, shift_idx, scale_idx,
+                            rows_per_frame, row_offset, q, ldq, scale_rows, static_cast<cudaStream_t>(stream));
+}
+
+int kr_gemm_i8_rowwise(int epilogue, const void* a, int lda, const void* w, int ldw, const float* scale_a,
+                       const float* scale_w, const void* bias, void* out, int ldc, int M, int N, int K,
+                       const void* residual, int ldr, const void* gate, int gate_stride, int rows_per_gate,
+                       void* out2, int ldc2, int n_split, int row_offset, void* stream) {
+  KR_REQUIRE(a && w && out, "null a/w/out");
+  KR_REQUIRE(scale_a && scale_w, "null scale_a/scale_w");
+  KR_REQUIRE_FP8_FAST_SHAPE();
+  KR_REQUIRE(K <= 132104, "K > 132104 could overflow the s32 sums");
+  KR_REQUIRE_LINKED(gemm_i8_rowwise_tn);
+  const kr::GemmParams p = gemm_params(bias, out, ldc, M, N, K, residual, ldr, gate, gate_stride, rows_per_gate, out2,
+                                       ldc2, n_split, row_offset);
+  return kr::gemm_i8_rowwise_tn(epilogue, a, lda, w, ldw, p, scale_a, scale_w, static_cast<cudaStream_t>(stream));
+}
+
 int kr_attn_fwd(int dtype, const void* q, int ldq, const void* k, int ldk, const void* v, int ldv,
                 void* out, int ldo, int Lq, int Lkv, int heads, float softmax_scale, int mask_mode,
                 int block_len, int window, int pad_keys, void* stream) {

@@ -155,8 +155,51 @@ KR_DEVICE void fp8_quantize_row_groups(const uint4 (&raw)[kVec], int nvec, uint8
   }
 }
 
+// Dynamic per-row symmetric s8 cast of one row held packed in registers by a kRowThreads CTA (torchao
+// Int8DynamicActivation, per token): amax = max(max|x|, 1e-12), q = clamp(rint(x * (127 / amax)), -127, 127) (round half
+// to even), scale_out = amax / 127.  `red` holds 4 floats; every thread of the CTA must call it.
+template <int kVec>
+KR_DEVICE void i8_quantize_row(const uint4 (&raw)[kVec], int nvec, float* red, int8_t* __restrict__ qrow,
+                               float* __restrict__ scale_out) {
+  float m = 0.f;
+#pragma unroll
+  for (int i = 0; i < kVec; ++i) {
+    const int vi = threadIdx.x + i * kRowThreads;
+    if (vi < nvec) {
+      const uint32_t u[4] = {raw[i].x, raw[i].y, raw[i].z, raw[i].w};
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        const float2 f = unpack_bf16x2(u[j]);
+        m = fmaxf(m, fmaxf(fabsf(f.x), fabsf(f.y)));
+      }
+    }
+  }
+  const float amax = fmaxf(block_max(m, red), 1e-12f);
+  const float mul = 127.0f / amax;
+  if (threadIdx.x == 0) *scale_out = amax / 127.0f;
+#pragma unroll
+  for (int i = 0; i < kVec; ++i) {
+    const int vi = threadIdx.x + i * kRowThreads;
+    if (vi < nvec) {
+      const uint32_t u[4] = {raw[i].x, raw[i].y, raw[i].z, raw[i].w};
+      uint32_t o[2] = {0u, 0u};
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        const float2 f = unpack_bf16x2(u[j]);
+        // the bounds are integers, so clamping before rounding equals clamping after
+        const int q0 = __float2int_rn(fminf(fmaxf(f.x * mul, -127.f), 127.f));
+        const int q1 = __float2int_rn(fminf(fmaxf(f.y * mul, -127.f), 127.f));
+        const uint32_t pair = (static_cast<uint32_t>(q0) & 0xffu) | ((static_cast<uint32_t>(q1) & 0xffu) << 8);
+        o[j >> 1] |= pair << (16 * (j & 1));
+      }
+      *reinterpret_cast<uint2*>(qrow + vi * 8) = make_uint2(o[0], o[1]);
+    }
+  }
+}
+
 // kBlocks (with kFp8): the cast is per 128-channel group (fp8_quantize_row_groups) into q / scale_rows[g * ld_s].
-template <int kVec, bool kFp8, bool kBlocks = false>
+// kI8 (with kFp8, which then names the quantised-output mode): the cast is the per-row s8 one (i8_quantize_row).
+template <int kVec, bool kFp8, bool kBlocks = false, bool kI8 = false>
 KR_DEVICE void ln_modulate_row(const uint16_t* __restrict__ x, int ldx, uint16_t* __restrict__ out, int ldo,
                                int D, float eps, const uint16_t* __restrict__ w, const uint16_t* __restrict__ b,
                                const uint16_t* __restrict__ mod, int mod_rows, int shift_idx, int scale_idx,
@@ -237,6 +280,9 @@ KR_DEVICE void ln_modulate_row(const uint16_t* __restrict__ x, int ldx, uint16_t
   }
   if constexpr (kFp8 && kBlocks)
     fp8_quantize_row_groups<kVec>(raw, nvec, q + static_cast<size_t>(row) * ldq, scale_rows + row, ld_s);
+  else if constexpr (kFp8 && kI8)
+    i8_quantize_row<kVec>(raw, nvec, red, reinterpret_cast<int8_t*>(q) + static_cast<size_t>(row) * ldq,
+                          scale_rows + row);
   else if constexpr (kFp8)
     fp8_quantize_row<kVec>(raw, nvec, red, q + static_cast<size_t>(row) * ldq, scale_rows + row);
 }
@@ -271,6 +317,17 @@ ln_modulate_fp8_blocks_kernel(const uint16_t* __restrict__ x, int ldx, uint16_t*
                               float* __restrict__ scale, int ld_s) {
   ln_modulate_row<kVec, true, true>(x, ldx, out, ldo, D, eps, w, b, mod, mod_rows, shift_idx, scale_idx,
                                     rows_per_frame, row_offset, q, ldq, scale, ld_s);
+}
+
+template <int kVec>
+__global__ void __launch_bounds__(kRowThreads, 8)
+ln_modulate_i8_kernel(const uint16_t* __restrict__ x, int ldx, uint16_t* __restrict__ out, int ldo,
+                      int D, float eps, const uint16_t* __restrict__ w, const uint16_t* __restrict__ b,
+                      const uint16_t* __restrict__ mod, int mod_rows, int shift_idx, int scale_idx,
+                      int rows_per_frame, int row_offset, uint8_t* __restrict__ q, int ldq,
+                      float* __restrict__ scale_rows) {
+  ln_modulate_row<kVec, true, false, true>(x, ldx, out, ldo, D, eps, w, b, mod, mod_rows, shift_idx, scale_idx,
+                                           rows_per_frame, row_offset, q, ldq, scale_rows);
 }
 
 static int ln_check(const char* who, int rows, int D, int ldx, int ldo, const void* w, const void* b, const void* mod,
@@ -349,6 +406,35 @@ int ln_modulate_fp8(const void* x, int ldx, void* out, int ldo, int rows, int D,
   }
 #undef KR_LN_LAUNCH
   return launch_status("ln_modulate_fp8");
+}
+
+int ln_modulate_i8(const void* x, int ldx, void* out, int ldo, int rows, int D, float eps,
+                   const void* w, const void* b, const void* mod, int mod_rows, int shift_idx,
+                   int scale_idx, int rows_per_frame, int row_offset, void* q, int ldq, float* scale_rows,
+                   cudaStream_t stream) {
+  const int rc = ln_check("ln_modulate_i8", rows, D, ldx, out != nullptr ? ldo : 8, w, b, mod, rows_per_frame);
+  if (rc != KR_OK) return rc;
+  if (ldq % 8 != 0 || ldq < D) {
+    set_last_error("ln_modulate_i8: unsupported ldq=%d for D=%d", ldq, D);
+    return KR_ERR_UNSUPPORTED_SHAPE;
+  }
+  const int nv = (D / 8 + kRowThreads - 1) / kRowThreads;
+#define KR_LN_LAUNCH(V)                                                                            \
+  ln_modulate_i8_kernel<V><<<rows, kRowThreads, 0, stream>>>(                                      \
+      static_cast<const uint16_t*>(x), ldx, static_cast<uint16_t*>(out), ldo, D, eps,              \
+      static_cast<const uint16_t*>(w), static_cast<const uint16_t*>(b),                            \
+      static_cast<const uint16_t*>(mod), mod_rows, shift_idx, scale_idx, rows_per_frame, row_offset, \
+      static_cast<uint8_t*>(q), ldq, scale_rows)
+  switch (nv) {
+    case 1: KR_LN_LAUNCH(1); break;
+    case 2: KR_LN_LAUNCH(2); break;
+    case 3: KR_LN_LAUNCH(3); break;
+    case 4: KR_LN_LAUNCH(4); break;
+    case 5: KR_LN_LAUNCH(5); break;
+    default: KR_LN_LAUNCH(8); break;
+  }
+#undef KR_LN_LAUNCH
+  return launch_status("ln_modulate_i8");
 }
 
 int ln_modulate_fp8_blocks(const void* x, int ldx, void* out, int ldo, int rows, int D, float eps,
@@ -430,6 +516,51 @@ int fp8_quantize_rows(const void* x, int ldx, int rows, int cols, void* q, int l
   }
 #undef KR_Q_LAUNCH
   return launch_status("fp8_quantize_rows");
+}
+
+// Dynamic per-row symmetric s8 activation cast (torchao Int8DynamicActivation, per token): the e4m3 row quantiser's
+// layout, i8_quantize_row's numerics; scale_rows[r] = amax_r / 127 is the row scale of the s8 GEMM.
+template <int kVec>
+__global__ void __launch_bounds__(kRowThreads)
+i8_quantize_rows_kernel(const uint16_t* __restrict__ x, int ldx, int cols, int8_t* __restrict__ q, int ldq,
+                        float* __restrict__ scale_rows) {
+  __shared__ float red[4];
+  const int row = blockIdx.x;
+  const uint16_t* xr = x + static_cast<size_t>(row) * ldx;
+  const int nvec = cols >> 3;
+  uint4 raw[kVec];
+#pragma unroll
+  for (int i = 0; i < kVec; ++i) {
+    const int vi = threadIdx.x + i * kRowThreads;
+    if (vi < nvec) raw[i] = *reinterpret_cast<const uint4*>(xr + vi * 8);
+  }
+  i8_quantize_row<kVec>(raw, nvec, red, q + static_cast<size_t>(row) * ldq, scale_rows + row);
+}
+
+int i8_quantize_rows(const void* x, int ldx, int rows, int cols, void* q, int ldq, float* scale_rows,
+                     cudaStream_t stream) {
+  if (cols <= 0 || cols % 8 != 0 || cols > kRowThreads * 8 * kQuantMaxVec || rows <= 0 || ldx % 8 != 0 ||
+      ldq % 8 != 0 || ldx < cols || ldq < cols) {
+    set_last_error("i8_quantize_rows: unsupported rows=%d cols=%d ldx=%d ldq=%d", rows, cols, ldx, ldq);
+    return KR_ERR_UNSUPPORTED_SHAPE;
+  }
+  const int nv = (cols / 8 + kRowThreads - 1) / kRowThreads;
+#define KR_Q_LAUNCH(V)                                                                             \
+  i8_quantize_rows_kernel<V><<<rows, kRowThreads, 0, stream>>>(                                    \
+      static_cast<const uint16_t*>(x), ldx, cols, static_cast<int8_t*>(q), ldq, scale_rows)
+  switch (nv) {
+    case 1: KR_Q_LAUNCH(1); break;
+    case 2: KR_Q_LAUNCH(2); break;
+    case 3: KR_Q_LAUNCH(3); break;
+    case 4: KR_Q_LAUNCH(4); break;
+    case 5: KR_Q_LAUNCH(5); break;
+    case 6: KR_Q_LAUNCH(6); break;
+    case 7: case 8: KR_Q_LAUNCH(8); break;
+    case 9: case 10: KR_Q_LAUNCH(10); break;
+    default: KR_Q_LAUNCH(14); break;
+  }
+#undef KR_Q_LAUNCH
+  return launch_status("i8_quantize_rows");
 }
 
 // Dynamic per-group e4m3 activation cast (torchao PerBlock [1, 128]): the row quantiser's CTA-per-row layout, one

@@ -110,10 +110,13 @@ KR_DEVICE void gemm_epilogue_row(float (&v)[kW], const int row, const int col0, 
     }
 }
 
-// 0 = bf16, 1 = fp16, 2 = e4m3 (K-major operands, 128-byte rows: 64 16-bit or 128 8-bit elements per k-block)
+// 0 = bf16, 1 = fp16, 2 = e4m3, 3 = s8 (K-major operands, 128-byte rows: 64 16-bit or 128 8-bit elements per
+// k-block).  s8 accumulates exact s32 sums, held bit for bit in the fp32 accumulator registers until the caller
+// converts them.
 template <int BN, int kKind>
 KR_DEVICE void gemm_k_step(float (&acc)[BN / 2], uint64_t a_desc, uint64_t b_desc, int scale_d) {
-  if constexpr (kKind == 2) wgmma_ss_e4m3<BN>(acc, a_desc, b_desc, scale_d);
+  if constexpr (kKind == 3) wgmma_ss_s8<BN>(reinterpret_cast<int32_t*>(acc), a_desc, b_desc, scale_d);
+  else if constexpr (kKind == 2) wgmma_ss_e4m3<BN>(acc, a_desc, b_desc, scale_d);
   else wgmma_ss<BN, kKind == 0, 0>(acc, a_desc, b_desc, scale_d);
 }
 
@@ -246,7 +249,9 @@ constexpr int kEpiScrFloats = 16 * kEpiScrPitch;       // one warp's 16 x 32 tra
 // The fragment of one warp (rows row0 .. row0+15 of the output, columns col_base + [0, BN)) -> fused epilogue.
 // Only the first n_valid columns (a multiple of 32) are stored; every accumulator is multiplied by `scale`, or, with
 // kRowScale, by row_scale[row] and then by col_scale[col] (the row-scaled FP8 GEMM; rows >= M read no row scale).
-template <int BN, bool kBf16, int kEpi, bool kRowScale = false>
+// kS32: the accumulators hold s32 sums bit for bit (the s8 GEMM); each is converted to fp32 (round to nearest) as it
+// leaves the transpose, 16 at a time, so no second copy of the fragment is live.
+template <int BN, bool kBf16, int kEpi, bool kRowScale = false, bool kS32 = false>
 KR_DEVICE void gemm_frag_epilogue(const float (&acc)[BN / 2], float* scr, int row0, int col_base, int n_valid,
                                   float scale, const GemmParams& p, const float* __restrict__ row_scale = nullptr,
                                   const float* __restrict__ col_scale = nullptr) {
@@ -278,7 +283,10 @@ KR_DEVICE void gemm_frag_epilogue(const float (&acc)[BN / 2], float* scr, int ro
         float v[16];
 #pragma unroll
         for (int q = 0; q < 4; ++q) {
-          const float4 f = *reinterpret_cast<const float4*>(scr + (lane >> 1) * kEpiScrPitch + half * 16 + q * 4);
+          float4 f = *reinterpret_cast<const float4*>(scr + (lane >> 1) * kEpiScrPitch + half * 16 + q * 4);
+          if constexpr (kS32)
+            f = make_float4(static_cast<float>(__float_as_int(f.x)), static_cast<float>(__float_as_int(f.y)),
+                            static_cast<float>(__float_as_int(f.z)), static_cast<float>(__float_as_int(f.w)));
           if constexpr (kRowScale) {
             const float4 sw = __ldg(reinterpret_cast<const float4*>(col_scale + col_base + c * 32 + half * 16) + q);
             v[4 * q] = f.x * sa * sw.x; v[4 * q + 1] = f.y * sa * sw.y;

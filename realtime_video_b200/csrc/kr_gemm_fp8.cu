@@ -26,6 +26,8 @@
 //   fast     (torch._scaled_mm(use_fast_accum=True)): the wgmma accumulates in place across the whole K with one group
 //            in flight, like the 16-bit GEMM, on a 128 x 256 tile (m64n256k32, half the shared-memory operand bytes
 //            per FLOP) without draining the tensor cores after every k-block.
+// gemm_i8_kernel<kEpi> (torchao Int8DynamicActivationInt8WeightConfig, oracle/int8_oracle.py) shares the body: the fast
+// structure with s8 operands, exact s32 sums and the row-scaled epilogue.
 #include "kr_common.cuh"
 #include "kr_gemm_epi.cuh"
 #include "kr_ops.h"
@@ -44,6 +46,7 @@ constexpr int f8_smem(bool fast) { return F8_STAGES * (F8_A_BYTES + f8_bn(fast) 
 static_assert(f8_smem(true) <= 227 * 1024, "4 stages of 16 KB A + 32 KB W and the epilogue scratch fit one SM");
 
 enum Fp8Scale { F8_SCALE_TENSOR, F8_SCALE_ROW, F8_SCALE_BLOCK };
+constexpr int kI8MaxK = 132104;   // 127 * 128 * K < 2^31
 
 // The I-th scale argument: a mode's scale arguments are separate kernel parameters, as many as the mode needs.
 template <int I, typename T, typename... R>
@@ -53,14 +56,17 @@ __host__ __device__ __forceinline__ auto f8_arg(T t, R... r) {
 }
 }  // namespace
 
+// The body of both 8-bit GEMM kernels.  kKind 2 = e4m3 (gemm_fp8_kernel); 3 = s8 (gemm_i8_kernel: row scales on the
+// fast structure, exact s32 sums converted to fp32 by the row-scaled epilogue).
 // The scale arguments by kScale.  tensor: scale_a -> one fp32, float scale_w.  row: scale_a -> [M], scale_w -> [N].
 // block: scale_a -> fp32 [K/128, ld_sa] (k-block-major: one k-block's row scales are contiguous), then long ld_sa and
 // scale_w -> fp32 [N/128, K/128].
-template <int kEpi, int kScale, bool kFast, typename... ScaleW>
-__global__ void __launch_bounds__(F8_THREADS, 1)
-gemm_fp8_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
-                const GemmParams p, const float* __restrict__ scale_a, ScaleW... scale_w) {
+template <int kKind, int kEpi, int kScale, bool kFast, typename... ScaleW>
+__device__ __forceinline__ void gemm_8bit_body(const CUtensorMap& tmap_a, const CUtensorMap& tmap_b,
+                                               const GemmParams p, const float* __restrict__ scale_a,
+                                               ScaleW... scale_w) {
   static_assert(!(kFast && kScale == F8_SCALE_BLOCK), "block scales are applied at the promotion");
+  static_assert(kKind == 2 || (kFast && kScale == F8_SCALE_ROW), "s8 sums are exact: in place, row scales only");
   constexpr int BN = f8_bn(kFast), B_BYTES = BN * F8_BK, STAGE_BYTES = F8_A_BYTES + B_BYTES;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
@@ -132,15 +138,32 @@ gemm_fp8_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constan
       gemm_frag_epilogue<BN, true, kEpi>(acc, scr, row0, n_blk * BN, BN, 1.f, p);
     } else {
       float acc[BN / 2];
-      gemm_mainloop<BN, 2, 1, !kFast>(acc, a_base, b_base, F8_A_BYTES, B_BYTES, F8_STAGES, full_bar, empty_bar, stage,
-                                      phase, 0, num_k);
+      gemm_mainloop<BN, kKind, 1, !kFast>(acc, a_base, b_base, F8_A_BYTES, B_BYTES, F8_STAGES, full_bar, empty_bar,
+                                          stage, phase, 0, num_k);
       if constexpr (kScale == F8_SCALE_ROW)
-        gemm_frag_epilogue<BN, true, kEpi, true>(acc, scr, m_blk * F8_BM + wg * 64 + (warp & 3) * 16, n_blk * BN, BN,
-                                                 s, p, scale_a, f8_arg<0>(scale_w...));
+        gemm_frag_epilogue<BN, true, kEpi, true, kKind == 3>(acc, scr, m_blk * F8_BM + wg * 64 + (warp & 3) * 16,
+                                                             n_blk * BN, BN, s, p, scale_a, f8_arg<0>(scale_w...));
       else
         gemm_frag_epilogue<BN, true, kEpi>(acc, scr, m_blk * F8_BM + wg * 64 + (warp & 3) * 16, n_blk * BN, BN, s, p);
     }
   }
+}
+
+template <int kEpi, int kScale, bool kFast, typename... ScaleW>
+__global__ void __launch_bounds__(F8_THREADS, 1)
+gemm_fp8_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
+                const GemmParams p, const float* __restrict__ scale_a, ScaleW... scale_w) {
+  gemm_8bit_body<2, kEpi, kScale, kFast>(tmap_a, tmap_b, p, scale_a, scale_w...);
+}
+
+// INT8 (torchao Int8DynamicActivationInt8WeightConfig): s8 x s8 wgmma (m64n256k32) summing exactly in s32 across the
+// whole K, then v = (float(acc) * scale_a[m]) * scale_w[n] and the bf16 epilogue.  |acc| <= 127 * 128 * K < 2^31 for
+// K <= 132104, which the host checks.
+template <int kEpi>
+__global__ void __launch_bounds__(F8_THREADS, 1)
+gemm_i8_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
+               const GemmParams p, const float* __restrict__ scale_a, const float* __restrict__ scale_w) {
+  gemm_8bit_body<3, kEpi, F8_SCALE_ROW, true>(tmap_a, tmap_b, p, scale_a, scale_w);
 }
 
 // ---------------------------------------------------------------------------
@@ -220,11 +243,11 @@ int fp8_quantize(const void* x, long ld, int rows, int cols, void* q, long ldq, 
 // ---------------------------------------------------------------------------
 // host launcher
 // ---------------------------------------------------------------------------
-template <bool kFast, int kEpi, int kScale, typename... ScaleW>
+template <int kKind, bool kFast, int kEpi, int kScale, typename... ScaleW>
 static int launch_fp8(const void* a, int lda, const void* w, int ldw, const GemmParams& p, cudaStream_t stream,
                       const float* scale_a, ScaleW... scale_w) {
   constexpr int BN = f8_bn(kFast), SMEM = f8_smem(kFast);
-  constexpr const char* name = kScale == F8_SCALE_BLOCK ? "gemm_fp8_blockwise" : "gemm_fp8";
+  constexpr const char* name = kKind == 3 ? "gemm_i8" : kScale == F8_SCALE_BLOCK ? "gemm_fp8_blockwise" : "gemm_fp8";
   CUtensorMap ta, tb;
   // byte tensors: [rows, K] uint8, box [128 | 256 rows, 128 bytes], SWIZZLE_128B
   const uint64_t da[2] = {static_cast<uint64_t>(p.K), static_cast<uint64_t>(p.M)};
@@ -237,7 +260,10 @@ static int launch_fp8(const void* a, int lda, const void* w, int ldw, const Gemm
   const uint32_t bb[2] = {F8_BK, BN};
   rc = make_tmap_u8(&tb, w, 2, db, sb, bb, 128);
   if (rc != KR_OK) return rc;
-  const auto kern = gemm_fp8_kernel<kEpi, kScale, kFast, ScaleW...>;
+  const auto kern = [] {
+    if constexpr (kKind == 3) return gemm_i8_kernel<kEpi>;
+    else return gemm_fp8_kernel<kEpi, kScale, kFast, ScaleW...>;
+  }();
   static bool attr_set = false;
   if (!attr_set) {
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM);
@@ -259,14 +285,18 @@ static int launch_fp8(const void* a, int lda, const void* w, int ldw, const Gemm
   return KR_OK;
 }
 
-// The argument checks of every mode, then the kernel of the epilogue (EPI_F32 only with block scales).
-template <bool kFast, int kScale, typename... ScaleW>
+// The argument checks of every mode, then the kernel of the epilogue (EPI_F32 only with block scales or s8).
+template <bool kFast, int kScale, int kKind = 2, typename... ScaleW>
 static int gemm_fp8_any(const char* who, int epi, const void* a, int lda, const void* w, int ldw, const GemmParams& p,
                         cudaStream_t stream, const float* scale_a, ScaleW... scale_w) {
   if (p.M <= 0 || p.N <= 0 || p.K <= 0 || p.N % f8_bn(kFast) != 0 || p.K % 16 != 0 || lda % 16 != 0 ||
       ldw % 16 != 0 || p.ldc % 8 != 0) {
     set_last_error("%s: unsupported shape M=%d N=%d K=%d (need N %% %d == 0, K / ld %% 16 == 0)", who, p.M, p.N, p.K,
                    f8_bn(kFast));
+    return KR_ERR_UNSUPPORTED_SHAPE;
+  }
+  if (kKind == 3 && p.K > kI8MaxK) {
+    set_last_error("%s: K=%d > %d could overflow the s32 sums", who, p.K, kI8MaxK);
     return KR_ERR_UNSUPPORTED_SHAPE;
   }
   if ((epi == EPI_BIAS_GATE_RES || epi == EPI_BIAS_RES || epi == EPI_MUL) && p.residual == nullptr) {
@@ -301,14 +331,16 @@ static int gemm_fp8_any(const char* who, int epi, const void* a, int lda, const 
     }
   }
   switch (epi) {
-    case EPI_BIAS: return launch_fp8<kFast, EPI_BIAS, kScale>(a, lda, w, ldw, p, stream, scale_a, scale_w...);
-    case EPI_BIAS_GELU: return launch_fp8<kFast, EPI_BIAS_GELU, kScale>(a, lda, w, ldw, p, stream, scale_a, scale_w...);
+    case EPI_BIAS: return launch_fp8<kKind, kFast, EPI_BIAS, kScale>(a, lda, w, ldw, p, stream, scale_a, scale_w...);
+    case EPI_BIAS_GELU:
+      return launch_fp8<kKind, kFast, EPI_BIAS_GELU, kScale>(a, lda, w, ldw, p, stream, scale_a, scale_w...);
     case EPI_BIAS_GATE_RES:
-      return launch_fp8<kFast, EPI_BIAS_GATE_RES, kScale>(a, lda, w, ldw, p, stream, scale_a, scale_w...);
-    case EPI_BIAS_RES: return launch_fp8<kFast, EPI_BIAS_RES, kScale>(a, lda, w, ldw, p, stream, scale_a, scale_w...);
+      return launch_fp8<kKind, kFast, EPI_BIAS_GATE_RES, kScale>(a, lda, w, ldw, p, stream, scale_a, scale_w...);
+    case EPI_BIAS_RES:
+      return launch_fp8<kKind, kFast, EPI_BIAS_RES, kScale>(a, lda, w, ldw, p, stream, scale_a, scale_w...);
     case EPI_F32:
-      if constexpr (kScale == F8_SCALE_BLOCK)
-        return launch_fp8<kFast, EPI_F32, kScale>(a, lda, w, ldw, p, stream, scale_a, scale_w...);
+      if constexpr (kScale == F8_SCALE_BLOCK || kKind == 3)
+        return launch_fp8<kKind, kFast, EPI_F32, kScale>(a, lda, w, ldw, p, stream, scale_a, scale_w...);
       [[fallthrough]];
     default: set_last_error("%s: unsupported epilogue %d", who, epi); return KR_ERR_INVALID_ARG;
   }
@@ -338,6 +370,11 @@ int gemm_fp8_blockwise_tn(int epi, const void* a, int lda, const void* w, int ld
                           const float* scale_a, int ld_sa, const float* scale_w, cudaStream_t stream) {
   return gemm_fp8_any<false, F8_SCALE_BLOCK>("gemm_fp8_blockwise", epi, a, lda, w, ldw, p, stream, scale_a,
                                              static_cast<long>(ld_sa), scale_w);
+}
+
+int gemm_i8_rowwise_tn(int epi, const void* a, int lda, const void* w, int ldw, const GemmParams& p,
+                       const float* scale_a, const float* scale_w, cudaStream_t stream) {
+  return gemm_fp8_any<true, F8_SCALE_ROW, 3>("gemm_i8_rowwise", epi, a, lda, w, ldw, p, stream, scale_a, scale_w);
 }
 
 }  // namespace kr

@@ -81,6 +81,18 @@ __attribute__((weak)) int ln_modulate_fp8_blocks(const void* x, int ldx, void* o
 __attribute__((weak)) int gemm_fp8_blockwise_tn(int epi, const void* a, int lda, const void* w, int ldw,
                                                 const GemmParams& p, const float* scale_a, int ld_sa,
                                                 const float* scale_w, cudaStream_t stream);
+// INT8 (torchao Int8DynamicActivationInt8WeightConfig): the per-row symmetric s8 cast and the LayerNorm writing it
+// (kr_dit_elem.cu), and the s8 GEMM with exact s32 accumulation and [M] row / [N] channel scales (kr_gemm_fp8.cu;
+// N % 256 == 0, K <= 132104).  Weak for the same reason.
+__attribute__((weak)) int i8_quantize_rows(const void* x, int ldx, int rows, int cols, void* q, int ldq,
+                                           float* scale_rows, cudaStream_t stream);
+__attribute__((weak)) int ln_modulate_i8(const void* x, int ldx, void* out, int ldo, int rows, int D, float eps,
+                                         const void* w, const void* b, const void* mod, int mod_rows, int shift_idx,
+                                         int scale_idx, int rows_per_frame, int row_offset, void* q, int ldq,
+                                         float* scale_rows, cudaStream_t stream);
+__attribute__((weak)) int gemm_i8_rowwise_tn(int epi, const void* a, int lda, const void* w, int ldw,
+                                             const GemmParams& p, const float* scale_a, const float* scale_w,
+                                             cudaStream_t stream);
 // 2-CTA cluster variant (W multicast to both CTAs, 128x256 tile per CTA), kr_gemm2.cu; N % 256 == 0
 int gemm2_tn(int dtype, int epi, const void* a, int lda, const void* w, int ldw, const GemmParams& p,
              cudaStream_t stream);

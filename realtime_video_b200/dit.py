@@ -34,7 +34,11 @@ def _linear(x, lin: nn.Linear, **kw) -> torch.Tensor:
     when ``realtime_video_b200.fp8.quantize_`` attached quantised weights to the module, with the granularity it
     attached: per tensor, per row (``x`` may then be an ``ops.Fp8Rows`` the LayerNorm already cast) or per block (``x``
     may be an ``ops.Fp8Blocks``), and with the accumulation mode it recorded (``fast_accum`` is passed only when
-    chosen; block scaling is promoted only)."""
+    chosen; block scaling is promoted only).  INT8 weights (``Int8DynamicActivationInt8WeightConfig``) run the s8
+    GEMM, with ``x`` a bf16 activation or an ``ops.I8Rows``."""
+    q = getattr(lin, "_kr_i8", None)
+    if q is not None:
+        return ops.linear_i8(x, q[0], q[1], lin.bias, **kw)
     q = getattr(lin, "_kr_fp8", None)
     if q is None:
         return ops.gemm(x, lin.weight, lin.bias, **kw)
@@ -58,9 +62,16 @@ def _blockwise(*lins: nn.Module) -> bool:
     return all(fp8.is_blockwise(m) for m in lins)
 
 
+def _int8(*lins: nn.Module) -> bool:
+    """Every one of ``lins`` runs the INT8 GEMM: their common input can be cast to s8 once, by its producer."""
+    return all(fp8.is_int8(m) for m in lins)
+
+
 def _ln_fp8(lins, x, **kw):
-    """The LayerNorm feeding ``lins`` with its e4m3 cast fused in when they all take the same FP8 input: per 128-channel
-    group (PerBlock) or per row (PerRow); None when they do not."""
+    """The LayerNorm feeding ``lins`` with its cast fused in when they all take the same quantised input: s8 per row
+    (INT8), e4m3 per 128-channel group (PerBlock) or e4m3 per row (PerRow); None when they do not."""
+    if _int8(*lins):
+        return ops.ln_modulate_i8(x, **kw)
     if _blockwise(*lins):
         return ops.ln_modulate_fp8_blocks(x, **kw)
     if _rowwise(*lins):
@@ -428,7 +439,9 @@ class CausalWanModel(nn.Module):
         if cache is not None and cache["is_init"]:
             k, v = cache["k"], cache["v"]
         else:
-            if _blockwise(ca.k, ca.v):
+            if _int8(ca.k, ca.v):
+                ctx = ops.i8_quantize_rows(ctx)         # one per-row s8 cast of the prompt feeds both projections
+            elif _blockwise(ca.k, ca.v):
                 ctx = ops.fp8_quantize_blocks(ctx)      # one per-group cast of the prompt feeds both projections
             elif _rowwise(ca.k, ca.v):
                 ctx = ops.fp8_quantize_rows(ctx)        # one per-row cast of the prompt feeds both projections
@@ -454,7 +467,8 @@ class CausalWanModel(nn.Module):
                 # not inside a CUDA-graph capture: the scratch workspace is cached across calls and must not come from
                 # a capture's private memory pool
                 and not (x.is_cuda and torch.cuda.is_current_stream_capturing())
-                and not any(hasattr(m, "_kr_fp8") for m in (sa.to_qkv, sa.o, ca.q, ca.o, blk.ffn[0], blk.ffn[2])))
+                and not any(hasattr(m, "_kr_fp8") or hasattr(m, "_kr_i8")
+                            for m in (sa.to_qkv, sa.o, ca.q, ca.o, blk.ffn[0], blk.ffn[2])))
 
     def _block_one_call(self, blk: CausalWanAttentionBlock, x, e0, grid, kv_cache, crossattn_cache, current_start, mask):
         sa, ca = blk.self_attn, blk.cross_attn
@@ -493,9 +507,9 @@ class CausalWanModel(nn.Module):
         r0 = 0 if self.sp is None else self.sp.rank * x.shape[0]       # global index of my first row
         emod = ops.add_modulation(blk.modulation, e0)                    # [F, 6, D]
         sa, ca = blk.self_attn, blk.cross_attn
-        # PerRow / PerBlock FP8: a LayerNorm whose every consumer is a row- (block-) scaled FP8 linear writes e4m3
-        # bytes + row (group) scales instead of its bf16 output (ln_modulate_fp8[_blocks]); `buf` is the bf16 scratch
-        # row buffer while there is one
+        # PerRow / PerBlock FP8 and INT8: a LayerNorm whose every consumer is a row- (block-) scaled FP8 linear or an
+        # INT8 linear writes e4m3 / s8 bytes + row (group) scales instead of its bf16 output (ln_modulate_fp8[_blocks],
+        # ln_modulate_i8); `buf` is the bf16 scratch row buffer while there is one
         h = _ln_fp8((sa.to_qkv,) if sa.fused_projections else (sa.q, sa.k, sa.v), x, eps=blk.eps, mod=emod,
                     shift_idx=0, scale_idx=1, rows_per_frame=fs, row_offset=r0)
         buf = None

@@ -15,7 +15,8 @@ resolving to the reference checkout, independent of the ``sys.path`` order:
     torchao.quantization.quant_api -> realtime_video_b200.fp8       (quantize_, Float8DynamicActivationFloat8WeightConfig,
                                                                      PerTensor: the `enable_fp8` lines release_server.py:179-182;
                                                                      PerRow: the same lines with granularity=PerRow() also resolve;
-                                                                     PerBlock: granularity=[PerBlock([1, 128]), PerBlock([128, 128])])
+                                                                     PerBlock: granularity=[PerBlock([1, 128]), PerBlock([128, 128])];
+                                                                     Int8DynamicActivationInt8WeightConfig: the W8A8 INT8 config)
     torchao.float8.inference   -> realtime_video_b200.fp8           (Float8MMConfig, where torchao defines it: the same lines
                                                                      with mm_config=Float8MMConfig(use_fast_accum=True))
 
@@ -43,7 +44,7 @@ ALIASES = {
     "demo_utils.vae": "realtime_video_b200.vae",
     "wan.modules.causal_model": "realtime_video_b200.dit",
     # `enable_fp8: true` (release_server.py:179-182): quantize_ / Float8DynamicActivationFloat8WeightConfig / PerTensor
-    # (or PerRow, or PerBlock)
+    # (or PerRow, or PerBlock), and Int8DynamicActivationInt8WeightConfig
     "torchao.quantization.quant_api": "realtime_video_b200.fp8",
     # Float8MMConfig, the mm_config argument of the config above, under the module torchao defines it in
     "torchao.float8.inference": "realtime_video_b200.fp8",

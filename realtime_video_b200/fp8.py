@@ -34,11 +34,21 @@ promoted to fp32) fed by ``kr_ln_modulate_fp8_blocks`` or ``kr_fp8_quantize_bloc
 per k-block, so this granularity exists only with promoted accumulation: ``Float8MMConfig(use_fast_accum=True)`` with
 ``PerBlock`` raises ``NotImplementedError``, and ``KR_FP8_FAST_ACCUM=1`` does not apply to it.
 
+``Int8DynamicActivationInt8WeightConfig()`` is torchao's W8A8 INT8 config: symmetric per-token s8 activations
+(q = clamp(rint(x * (127 / amax_r)), -127, 127), scale amax_r / 127), symmetric per-output-channel s8 weights
+(q = clamp(rint(w / s_n), -128, 127), s_n = amax_n / 127.5), and an s8 tensor-core GEMM whose s32 sums are exact.  The
+block schedule then runs ``kr_gemm_i8_rowwise`` (128 x 256 tile, in-place s32 accumulation, the bf16 GEMM's epilogues
+after v = (float(acc) * s_r) * s_n) fed by ``kr_ln_modulate_i8`` or ``kr_i8_quantize_rows``; oracle/int8_oracle.py
+restates it.  Against e4m3 PerRow it trades accuracy on heavy tails and channel outliers (a uniform grid of 255 steps)
+for accuracy on bounded activations (3 mantissa bits); see DESIGN.md section 5.  INT8 and FP8 attachments exclude each
+other: quantising a module with one tier replaces the other's.
+
 Numerics are a separate tier from the bf16 headline: e4m3 has 3 mantissa bits; tests state the tolerance against the
 fp8 oracle (same quantisation, fp32 matmul) and against the bf16 path.
 """
 from __future__ import annotations
 
+import enum
 import os
 from dataclasses import dataclass
 
@@ -139,6 +149,43 @@ class Float8DynamicActivationFloat8WeightConfig:
         return g[0]
 
 
+class MappingType(enum.Enum):
+    """torchao.quantization.quant_primitives.MappingType: how a quantised range maps onto the real line."""
+    SYMMETRIC = enum.auto()
+    SYMMETRIC_NO_CLIPPING_ERR = enum.auto()
+    ASYMMETRIC = enum.auto()
+
+
+class PlainLayout:
+    """torchao's default tensor layout (torchao.dtypes.PlainLayout): the quantised weight stored as a dense [N, K]."""
+
+
+I8_MAX_K = 132104   # 127 * 128 * K < 2^31: the s32 sums of the INT8 GEMM cannot overflow
+
+
+class Int8DynamicActivationInt8WeightConfig:
+    """torchao's W8A8 INT8 config: per-token symmetric s8 activations, per-channel symmetric s8 weights.  Only the
+    defaults are implemented: ``layout`` None or :class:`PlainLayout`, ``act_mapping_type`` ``MappingType.SYMMETRIC``
+    and ``weight_only_decode=False`` (anything else raises ``NotImplementedError``).  ``set_inductor_config`` is
+    accepted and has nothing to configure here."""
+
+    def __init__(self, layout=None, act_mapping_type=MappingType.SYMMETRIC, weight_only_decode=False,
+                 set_inductor_config=True):
+        if layout is not None and type(layout) is not PlainLayout:
+            raise NotImplementedError(f"Int8DynamicActivationInt8WeightConfig: layout {type(layout).__name__} is not "
+                                      "implemented (PlainLayout)")
+        if act_mapping_type is not MappingType.SYMMETRIC:
+            raise NotImplementedError(f"Int8DynamicActivationInt8WeightConfig: act_mapping_type {act_mapping_type} "
+                                      "is not implemented (MappingType.SYMMETRIC)")
+        if weight_only_decode:
+            raise NotImplementedError("Int8DynamicActivationInt8WeightConfig: weight_only_decode=True is not "
+                                      "implemented")
+        self.layout = layout
+        self.act_mapping_type = act_mapping_type
+        self.weight_only_decode = weight_only_decode
+        self.set_inductor_config = set_inductor_config
+
+
 @torch.no_grad()
 def quantize_weight(w: torch.Tensor):
     """w [N, K] -> (e4m3 bytes as uint8 [N, K], dequantisation scale amax / 448): w_q = sat(w * 448 / amax)."""
@@ -172,6 +219,22 @@ def quantize_weight_blocks(w: torch.Tensor):
     return q.view(torch.uint8).contiguous(), (amax / E4M3_MAX).reshape(N // BLOCK, K // BLOCK).contiguous()
 
 
+@torch.no_grad()
+def quantize_weight_int8_rows(w: torch.Tensor):
+    """w [N, K] -> (int8 [N, K], fp32 [N] dequantisation scales s_n = amax_n / 127.5), symmetric over [-128, 127]:
+    w_q[n] = clamp(rint(w[n] / s_n), -128, 127) (round half to even).  An all-zero channel gets the scale
+    torch.finfo(float32).eps (torchao's floor), so it quantises to zeros."""
+    amax = w.detach().float().abs().amax(dim=1, keepdim=True)
+    scale = (amax / 127.5).clamp(min=torch.finfo(torch.float32).eps)
+    q = torch.round(w.detach().float() / scale).clamp(-128, 127).to(torch.int8)
+    return q.contiguous(), scale.squeeze(1).contiguous()
+
+
+def is_int8(lin: nn.Module) -> bool:
+    """True when :func:`quantize_` attached INT8 weights to ``lin``."""
+    return hasattr(lin, "_kr_i8")
+
+
 def is_rowwise(lin: nn.Module) -> bool:
     """True when :func:`quantize_` attached per-row (PerRow) FP8 weights to ``lin``."""
     return isinstance(getattr(lin, "_kr_fp8_granularity", None), PerRow)
@@ -194,7 +257,11 @@ def quantize_(module: nn.Module, config=None, filter_fn=None) -> nn.Module:
     (state_dict unchanged); call ``dequantize_`` to go back.  PerTensor attaches ``(w_q, scale_w float)``, PerRow
     ``(w_q, scale_w fp32 [N])``, PerBlock ``(w_q, scale_w fp32 [N/128, K/128])`` (only to Linears with K % 128 == 0)
     on the weight's device.  The accumulation mode of ``config.mm_config`` is recorded
-    beside them; the weights and scales do not depend on it."""
+    beside them; the weights and scales do not depend on it.  :class:`Int8DynamicActivationInt8WeightConfig` attaches
+    ``(w_q int8, scale_w fp32 [N])`` instead (only to Linears with K <= 132104).  Either replaces what an earlier call
+    with the other tier attached."""
+    if isinstance(config, Int8DynamicActivationInt8WeightConfig):
+        return _quantize_int8(module, filter_fn)
     if config is not None and not isinstance(config, Float8DynamicActivationFloat8WeightConfig):
         raise NotImplementedError(f"unsupported quantisation config {type(config).__name__}")
     gran = config.granularity if config is not None else PerTensor()
@@ -211,6 +278,7 @@ def quantize_(module: nn.Module, config=None, filter_fn=None) -> nn.Module:
         for name, lin in blk.named_modules():
             if isinstance(lin, nn.Linear) and lin.weight.shape[0] % 256 == 0 and lin.weight.shape[1] % 16 == 0 and \
                     (not blocks or lin.weight.shape[1] % BLOCK == 0) and (filter_fn is None or filter_fn(lin, name)):
+                _detach(lin, _I8_ATTRS)
                 lin._kr_fp8 = quant(lin.weight)
                 lin._kr_fp8_granularity = gran
                 if fast:
@@ -223,11 +291,36 @@ def quantize_(module: nn.Module, config=None, filter_fn=None) -> nn.Module:
     return module
 
 
+_FP8_ATTRS = ("_kr_fp8", "_kr_fp8_granularity", "_kr_fp8_fast_accum")
+_I8_ATTRS = ("_kr_i8",)
+
+
+def _detach(lin: nn.Module, attrs) -> None:
+    for attr in attrs:
+        if hasattr(lin, attr):
+            delattr(lin, attr)
+
+
+def _quantize_int8(module: nn.Module, filter_fn) -> nn.Module:
+    from .dit import CausalWanAttentionBlock
+    n = 0
+    for blk in module.modules():
+        if not isinstance(blk, CausalWanAttentionBlock):
+            continue
+        for name, lin in blk.named_modules():
+            N, K = lin.weight.shape if isinstance(lin, nn.Linear) else (0, 0)
+            if isinstance(lin, nn.Linear) and N % 256 == 0 and K % 16 == 0 and K <= I8_MAX_K and \
+                    (filter_fn is None or filter_fn(lin, name)):
+                _detach(lin, _FP8_ATTRS)
+                lin._kr_i8 = quantize_weight_int8_rows(lin.weight)
+                n += 1
+    if n == 0:
+        raise ValueError("quantize_: no DiT block linears found in the module")
+    return module
+
+
 def dequantize_(module: nn.Module) -> nn.Module:
     for lin in module.modules():
-        if isinstance(lin, nn.Linear) and hasattr(lin, "_kr_fp8"):
-            del lin._kr_fp8
-            for attr in ("_kr_fp8_granularity", "_kr_fp8_fast_accum"):
-                if hasattr(lin, attr):
-                    delattr(lin, attr)
+        if isinstance(lin, nn.Linear):
+            _detach(lin, _FP8_ATTRS + _I8_ATTRS)
     return module

@@ -247,15 +247,16 @@ _fp8_scratch = {}
 
 
 def _fp8_cast_scratch(kind: str, x: torch.Tensor):
-    """``x`` as [rows, cols] and the (q, scale) buffers its ``kind`` ("tensor", "rows" or "blocks") FP8 cast writes,
+    """``x`` as [rows, cols] and the (q, scale) buffers its ``kind`` ("tensor", "rows", "blocks" or "i8") cast writes,
     reused per (kind, device, rows, cols); the launches are stream-ordered."""
     rows, _ = _rows2d(x, "x")
     cols = x.shape[-1]
     key = (kind, x.device.index, rows, cols)
     sc = _fp8_scratch.get(key)
     if sc is None:
-        scale_shape = {"tensor": (2,), "rows": (rows,), "blocks": (cols // 128, rows)}[kind]
-        sc = _fp8_scratch[key] = (torch.empty(rows, cols, dtype=torch.uint8, device=x.device),
+        scale_shape = {"tensor": (2,), "rows": (rows,), "blocks": (cols // 128, rows), "i8": (rows,)}[kind]
+        qtype = torch.int8 if kind == "i8" else torch.uint8
+        sc = _fp8_scratch[key] = (torch.empty(rows, cols, dtype=qtype, device=x.device),
                                   torch.empty(scale_shape, dtype=torch.float32, device=x.device))
     return (x if x.dim() == 2 else x.reshape(rows, -1)), *sc
 
@@ -335,14 +336,16 @@ class Fp8Rows(NamedTuple):
         return self.q.device
 
 
-def _rows_out(rows: int, cols: int, device, q: Optional[torch.Tensor], scale: Optional[torch.Tensor]):
+def _rows_out(rows: int, cols: int, device, q: Optional[torch.Tensor], scale: Optional[torch.Tensor],
+              qtype: torch.dtype = torch.uint8):
     if q is None:
-        q = torch.empty(rows, cols, dtype=torch.uint8, device=device)
+        q = torch.empty(rows, cols, dtype=qtype, device=device)
     if scale is None:
         scale = torch.empty(rows, dtype=torch.float32, device=device)
-    _req(q, "q", torch.uint8); _req(scale, "scale", torch.float32)
+    _req(q, "q", qtype); _req(scale, "scale", torch.float32)
     if q.shape[0] < rows or q.shape[-1] < cols or q.stride(-1) != 1 or scale.numel() < rows or not scale.is_contiguous():
-        raise _lib.KreaB200Error(f"fp8 rows: q must be [>= {rows}, >= {cols}] with contiguous rows and scale [>= {rows}]")
+        raise _lib.KreaB200Error(f"quantised rows: q must be [>= {rows}, >= {cols}] with contiguous rows and scale "
+                                 f"[>= {rows}]")
     return q, scale
 
 
@@ -368,8 +371,8 @@ def ln_modulate_fp8(x: torch.Tensor, *, eps: float, weight: Optional[torch.Tenso
                     scale: Optional[torch.Tensor] = None) -> Fp8Rows:
     """:func:`ln_modulate` whose output rows are cast to e4m3 per row in the same kernel (exactly
     :func:`fp8_quantize_rows` of the bf16 output).  The bf16 output is written only when ``out`` is given."""
-    return _ln_modulate_fp8(False, x, eps, weight, bias, mod, shift_idx, scale_idx, rows_per_frame, out, row_offset,
-                            q, scale)
+    return _ln_modulate_q("fp8", x, eps, weight, bias, mod, shift_idx, scale_idx, rows_per_frame, out, row_offset,
+                          q, scale)
 
 
 def gemm_fp8_rowwise(a: Fp8Rows, w_q: torch.Tensor, scale_w: torch.Tensor, bias: Optional[torch.Tensor] = None, *,
@@ -443,10 +446,12 @@ def _blocks_out(rows: int, cols: int, device, q: Optional[torch.Tensor], scale: 
     return q, scale
 
 
-def _ln_modulate_fp8(blocks: bool, x: torch.Tensor, eps: float, weight, bias, mod, shift_idx: int, scale_idx: int,
-                     rows_per_frame: int, out, row_offset: int, q, scale):
-    """The body of :func:`ln_modulate_fp8` (per-row cast) and :func:`ln_modulate_fp8_blocks` (per-group cast)."""
-    name = "ln_modulate_fp8_blocks" if blocks else "ln_modulate_fp8"
+def _ln_modulate_q(cast: str, x: torch.Tensor, eps: float, weight, bias, mod, shift_idx: int, scale_idx: int,
+                   rows_per_frame: int, out, row_offset: int, q, scale):
+    """The body of :func:`ln_modulate_fp8` (``cast`` "fp8": per-row e4m3), :func:`ln_modulate_fp8_blocks`
+    ("fp8_blocks": per-group e4m3) and :func:`ln_modulate_i8` ("i8": per-row s8)."""
+    name = "ln_modulate_" + cast
+    blocks = cast == "fp8_blocks"
     _req(x, "x", torch.bfloat16)
     rows, ldx = _rows2d(x, "x")
     D = x.shape[-1]
@@ -460,7 +465,10 @@ def _ln_modulate_fp8(blocks: bool, x: torch.Tensor, eps: float, weight, bias, mo
         if not mod.is_contiguous() or mod.shape[-1] != D:
             raise _lib.KreaB200Error(f"{name}: mod must be contiguous [frames, rows, D]")
         mod_rows = mod.shape[-2]
-    q, scale = (_blocks_out if blocks else _rows_out)(rows, D, x.device, q, scale)
+    if blocks:
+        q, scale = _blocks_out(rows, D, x.device, q, scale)
+    else:
+        q, scale = _rows_out(rows, D, x.device, q, scale, torch.int8 if cast == "i8" else torch.uint8)
     ld_s = (scale.stride(0),) if blocks else ()
     lib = _lib.load()
     rc = getattr(lib, "kr_" + name)(x.data_ptr(), ldx, _ptr(out), ldo, rows, D, eps, _ptr(weight), _ptr(bias),
@@ -468,7 +476,7 @@ def _ln_modulate_fp8(blocks: bool, x: torch.Tensor, eps: float, weight, bias, mo
                                     q.data_ptr(), q.stride(0), scale.data_ptr(), *ld_s, _stream())
     _lib.check(rc, "kr_" + name)
     _count()
-    return (Fp8Blocks if blocks else Fp8Rows)(q, scale, x.dtype)
+    return {"fp8": Fp8Rows, "fp8_blocks": Fp8Blocks, "i8": I8Rows}[cast](q, scale, x.dtype)
 
 
 def fp8_quantize_blocks(x: torch.Tensor, q: Optional[torch.Tensor] = None,
@@ -494,8 +502,8 @@ def ln_modulate_fp8_blocks(x: torch.Tensor, *, eps: float, weight: Optional[torc
                            scale: Optional[torch.Tensor] = None) -> Fp8Blocks:
     """:func:`ln_modulate` whose output rows are cast to e4m3 per 128-channel group in the same kernel (exactly
     :func:`fp8_quantize_blocks` of the bf16 output).  The bf16 output is written only when ``out`` is given."""
-    return _ln_modulate_fp8(True, x, eps, weight, bias, mod, shift_idx, scale_idx, rows_per_frame, out, row_offset,
-                            q, scale)
+    return _ln_modulate_q("fp8_blocks", x, eps, weight, bias, mod, shift_idx, scale_idx, rows_per_frame, out,
+                          row_offset, q, scale)
 
 
 def gemm_fp8_blockwise(a: Fp8Blocks, w_q: torch.Tensor, scale_w: torch.Tensor, bias: Optional[torch.Tensor] = None,
@@ -537,6 +545,86 @@ def linear_fp8_blockwise(x, w_q: torch.Tensor, scale_w: torch.Tensor, bias: Opti
     if not isinstance(x, Fp8Blocks):
         x = fp8_quantize_blocks(*_fp8_cast_scratch("blocks", x))
     return gemm_fp8_blockwise(x, w_q, scale_w, bias, **kw)
+
+
+class I8Rows(NamedTuple):
+    """A row-quantised s8 activation standing in for the 16-bit tensor it was cast from (torchao
+    Int8DynamicActivation, per token): ``q`` int8 [rows, cols], dequantisation scales ``scale`` fp32 [rows] =
+    amax_r / 127, and the ``dtype`` of the source tensor."""
+    q: torch.Tensor
+    scale: torch.Tensor
+    dtype: torch.dtype
+
+    @property
+    def shape(self):
+        return self.q.shape
+
+    @property
+    def device(self):
+        return self.q.device
+
+
+def i8_quantize_rows(x: torch.Tensor, q: Optional[torch.Tensor] = None,
+                     scale: Optional[torch.Tensor] = None) -> I8Rows:
+    """Dynamic per-row symmetric s8 cast (torchao Int8DynamicActivation): x [rows, cols] bf16 (row pitch free) ->
+    I8Rows(q int8 [rows, cols] = clamp(rint(x * (127 / amax_r)), -127, 127), scale fp32 [rows] = amax_r / 127)."""
+    _req(x, "x", torch.bfloat16)
+    rows, ld = _rows2d(x, "x")
+    cols = x.shape[-1]
+    q, scale = _rows_out(rows, cols, x.device, q, scale, torch.int8)
+    lib = _lib.load()
+    rc = lib.kr_i8_quantize_rows(x.data_ptr(), ld, rows, cols, q.data_ptr(), q.stride(0), scale.data_ptr(), _stream())
+    _lib.check(rc, "kr_i8_quantize_rows")
+    _count()
+    return I8Rows(q, scale, x.dtype)
+
+
+def ln_modulate_i8(x: torch.Tensor, *, eps: float, weight: Optional[torch.Tensor] = None,
+                   bias: Optional[torch.Tensor] = None, mod: Optional[torch.Tensor] = None,
+                   shift_idx: int = 0, scale_idx: int = 1, rows_per_frame: int = 0,
+                   out: Optional[torch.Tensor] = None, row_offset: int = 0, q: Optional[torch.Tensor] = None,
+                   scale: Optional[torch.Tensor] = None) -> I8Rows:
+    """:func:`ln_modulate` whose output rows are cast to s8 per row in the same kernel (exactly
+    :func:`i8_quantize_rows` of the bf16 output).  The bf16 output is written only when ``out`` is given."""
+    return _ln_modulate_q("i8", x, eps, weight, bias, mod, shift_idx, scale_idx, rows_per_frame, out, row_offset,
+                          q, scale)
+
+
+def gemm_i8_rowwise(a: I8Rows, w_q: torch.Tensor, scale_w: torch.Tensor, bias: Optional[torch.Tensor] = None, *,
+                    epilogue: int = EPI_BIAS, out: Optional[torch.Tensor] = None,
+                    residual: Optional[torch.Tensor] = None, gate: Optional[torch.Tensor] = None,
+                    rows_per_gate: int = 0, out2: Optional[torch.Tensor] = None, n_split: int = 0,
+                    row_offset: int = 0) -> torch.Tensor:
+    """out[M,N] = epilogue((float(a.q[M,K] @ w_q[N,K]^T) * a.scale[m]) * scale_w[n] + bias), the product summed
+    exactly in s32; w_q int8, scale_w fp32 [N].  bf16 output, or fp32 with ``epilogue=EPI_F32``."""
+    _req(a.q, "a.q", torch.int8); _req(a.scale, "a.scale", torch.float32)
+    _req(w_q, "w_q", torch.int8); _req(scale_w, "scale_w", torch.float32)
+    M, K = a.q.shape
+    N = w_q.shape[0]
+    if w_q.shape[1] != K or scale_w.numel() != N or not scale_w.is_contiguous() or a.scale.numel() < M:
+        raise _lib.KreaB200Error(f"gemm_i8_rowwise: w_q {tuple(w_q.shape)} / scale_w {tuple(scale_w.shape)} / "
+                                 f"a.scale {tuple(a.scale.shape)} do not match M={M} K={K}")
+    if out is None:
+        out = torch.empty(M, N, dtype=torch.float32 if epilogue == EPI_F32 else torch.bfloat16, device=a.q.device)
+    ldc, ldr, gs, ldc2 = _fp8_epi_pitches(out, residual, gate, out2)
+    lib = _lib.load()
+    with _Timed("gemm_i8", 2.0 * M * N * K):
+        rc = lib.kr_gemm_i8_rowwise(epilogue, a.q.data_ptr(), a.q.stride(0), w_q.data_ptr(), w_q.stride(0),
+                                    a.scale.data_ptr(), scale_w.data_ptr(), _ptr(bias), out.data_ptr(), ldc, M, N, K,
+                                    _ptr(residual), ldr, _ptr(gate), gs, rows_per_gate, _ptr(out2), ldc2, n_split,
+                                    row_offset, _stream())
+    _lib.check(rc, "kr_gemm_i8_rowwise")
+    _count()
+    return out
+
+
+def linear_i8(x, w_q: torch.Tensor, scale_w: torch.Tensor, bias: Optional[torch.Tensor] = None, **kw):
+    """INT8 dynamic-activation linear (torchao Int8DynamicActivationInt8WeightConfig): ``x`` is a bf16 activation
+    (cast per row here, into scratch reused per (device, rows, cols); the launches are stream-ordered) or an
+    :class:`I8Rows` already cast by :func:`ln_modulate_i8` / :func:`i8_quantize_rows`; then the s8 GEMM."""
+    if not isinstance(x, I8Rows):
+        x = i8_quantize_rows(*_fp8_cast_scratch("i8", x))
+    return gemm_i8_rowwise(x, w_q, scale_w, bias, **kw)
 
 
 def attention(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, *, heads: int,
